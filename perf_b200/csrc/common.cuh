@@ -409,6 +409,31 @@ __device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t adesc, uint64_t
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                  : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
 }
+
+// The same with A from REGISTERS (K-major, fp16 pairs): thread l of warp w holds a[0] = (row 16w + l/4, cols 2(l%4), +1),
+// a[1] = (row + 8, same cols), a[2] = (row, cols 8 + 2(l%4), +1), a[3] = (row + 8, cols 8 + 2(l%4), +1) -- the layout of
+// accumulator pairs (4j, 4j+1), (4j+2, 4j+3) of two neighbouring column groups j of an m64nN fp32 fragment (relu_frag).
+__device__ __forceinline__ void wgmma_n64_ra(float (&d)[32], const uint32_t* a, uint64_t bdesc, uint32_t accumulate)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+                 "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_n8_ra(float (&d)[4], const uint32_t* a, uint64_t bdesc, uint32_t accumulate)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %9, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 "
+                 "{%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 #endif  // __CUDACC__
 
 }  // namespace perf

@@ -3,7 +3,8 @@
 // One CTA = 128 threads = one warpgroup = one 128-row tile; thread t owns row t: it produces the row's fp16 input
 // features and runs the row's epilogue.  A layer is two M=64 wgmma chains (rows 0-63, 64-127) whose fp32 accumulator
 // fragments are rounded (ReLU, fp16) in registers and written straight into the next layer's operand image, from
-// which every thread then reads its own row back.
+// which every thread then reads its own row back (layer_relu).  The eval renders skip that round trip after layer 1: the
+// rounded fragments ARE the next layer's A operand in registers (relu_frag, render.cu::eval_mlp_regs).
 //
 // Operand layout in shared memory (both A = activations and B = weights): K-major, NO swizzle,
 // i.e. the canonical "interleaved" layout of 8x16-byte core matrices:
@@ -83,6 +84,14 @@ __device__ __forceinline__ void relu_pack(const float (&v)[32], uint32_t (&p)[16
 __device__ __forceinline__ uint32_t relu_pack2(float lo, float hi)
 {
     uint32_t p; asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(p) : "f"(hi), "f"(lo)); return p;
+}
+
+// m64n64 fp32 accumulator fragment -> ReLU-rounded fp16 A fragments of the next layer, without leaving the registers:
+// register j of k-slice s (a[4s + j], columns [16s, 16s + 16)) is the accumulator pair (8s + 2j, 8s + 2j + 1).
+__device__ __forceinline__ void relu_frag(const float (&d)[32], uint32_t (&a)[16])
+{
+#pragma unroll
+    for (int i = 0; i < 16; ++i) a[i] = relu_pack2(d[2 * i], d[2 * i + 1]);
 }
 
 // acc.x += a.x * b.x, acc.y += a.y * b.y: two independent fp32 FMAs (the even / odd partial sums of out_dots)
@@ -165,7 +174,8 @@ __device__ __forceinline__ void layer_relu(uint8_t* dst, const uint8_t* A, const
 // Output layer on CUDA cores (n_out is 1 or 3: a padded N=16 MMA + another smem round trip would cost more than the
 // 64*n_out FMAs per row).  Every output keeps TWO partial sums -- acc[o].x over the even hidden units, acc[o].y over
 // the odd ones, in increasing order -- one pair per packed pair of activations; the pre-activation is
-// acc[o].x + acc[o].y (out_sum).  All forward kernels share this order.
+// acc[o].x + acc[o].y (out_sum).  network_fwd_kernel, the training forward (render.cu, SAVE = 1/2), the SIMT twin and the
+// legacy scan kernel share this order; the eval renders (render.cu::eval_mlp_regs) sum the output layers on the tensor cores.
 //   acc[o] += h[32c + 2j, 32c + 2j + 1] * wout[o][32c + 2j, 32c + 2j + 1]      (wout: fp32 in shared memory)
 template <int NOUT_MAX>
 __device__ __forceinline__ void out_dots(const uint32_t (&p)[16], const float* wout, int c, int n_out, float2 (&acc)[NOUT_MAX])

@@ -61,30 +61,52 @@ struct RenderArgs {
     float*        s_toff;       // [seg * R] transmittance at the start of each segment (SAVE, seg > 1)
 };
 
+// Shared memory of the kernels that round-trip the hidden layers through shared memory: the training forward (SAVE = 1/2),
+// the SIMT twin and the legacy scan kernel.
 constexpr int RS_A     = 0;                         // 16 KB: A_geo | A_app, later the colour hidden layers (K=64)
 constexpr int RS_H     = RS_A + A64_BYTES;          // 16 KB: density hidden layer
 constexpr int RS_W1G   = RS_H + A64_BYTES;
 constexpr int RS_W1A   = RS_W1G + W32_BYTES;
 constexpr int RS_W2A   = RS_W1A + W32_BYTES;
-constexpr int RS_WOUT  = RS_W2A + W64_BYTES;        // fp32: geo [64] then app [3][64]
+constexpr int RS_WOUT  = RS_W2A + W64_BYTES;        // 1 KB, unused (the output weights are read from c_wout)
 constexpr int RS_TAILS = RS_WOUT + 4 * HID * 4;     // [2 scans][4 warps][8] floats
 constexpr int RS_CARRY = RS_TAILS + 2 * 4 * 8 * 4;  // [2 parities][8] floats
 constexpr int RS_BARW  = RS_CARRY + 2 * 8 * 4;     // mbarrier of the weight bulk copy
 constexpr int RS_TOTAL = RS_BARW + 16;
+constexpr int W_IMG_BYTES = W32_BYTES + W32_BYTES + W64_BYTES;       // 16 KB: W1 density | W1 colour | W2 colour
+static_assert(RS_W1A == RS_W1G + W32_BYTES && RS_W2A == RS_W1A + W32_BYTES, "the three weight images are one contiguous block");
+
+// Shared memory of the eval kernels (wgmma MLP, no saves: eval_mlp_regs): the feature tile and the weight images only --
+// the hidden layers never leave the registers.  ~34 KB, so 4 CTAs fit the 164 KB shared-memory carveout and leave 92 KB
+// of the SM's 256 KB to the L1 that serves the table gathers (the layout above needs the 228 KB carveout: 28 KB of L1).
+constexpr int WO_BYTES = 8 * HID * 2;               // 1 KB: an output layer as an N = 8 operand image (mlp_tc.cuh layout, LBO = 128)
+constexpr int WO_LBO   = 8 * 16;
+constexpr int RE_A     = 0;                         // 16 KB: A_geo | A_app
+constexpr int RE_W1G   = RE_A + A64_BYTES;
+constexpr int RE_W1A   = RE_W1G + W32_BYTES;
+constexpr int RE_W2A   = RE_W1A + W32_BYTES;
+constexpr int RE_WOG   = RE_W2A + W64_BYTES;        // density output row 0, rows 1-7 zero
+constexpr int RE_WOA   = RE_WOG + WO_BYTES;         // colour output rows 0-2, rows 3-7 zero
+constexpr int RE_MAX   = RE_WOA + WO_BYTES;         // [4 warps] longest packed ray (perf_render_packed)
+constexpr int RE_BARW  = RE_MAX + 16;               // mbarrier of the weight bulk copy
+constexpr int RE_TOTAL = RE_BARW + 16;
+constexpr int W_IMG_ALL = W_IMG_BYTES + 2 * WO_BYTES;                // 18 KB: the hidden images, then the two output images
+static_assert(RE_W1A == RE_W1G + W32_BYTES && RE_W2A == RE_W1A + W32_BYTES && RE_WOG == RE_W1G + W_IMG_BYTES &&
+              RE_WOA == RE_WOG + WO_BYTES, "the five weight images are one contiguous block");
+static_assert(4 * (RE_TOTAL + 1024) <= 164 * 1024, "4 eval CTAs (+1 KB reserved each) fit the 164 KB shared-memory carveout");
 // measurement hook (tools/ab_lib.py): extra, unused dynamic shared memory per CTA of the march kernels, i.e. what
 // more shared memory would cost in L1 capacity
 #ifndef PERF_RS_PAD
 #define PERF_RS_PAD 0
 #endif
 constexpr int RS_LAUNCH = RS_TOTAL + PERF_RS_PAD;
-constexpr int W_IMG_BYTES = W32_BYTES + W32_BYTES + W64_BYTES;       // 16 KB: W1 density | W1 colour | W2 colour
-static_assert(RS_W1A == RS_W1G + W32_BYTES && RS_W2A == RS_W1A + W32_BYTES, "the three weight images are one contiguous block");
-// experiment (PERF_FLAG_L0_SMEM): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared memory,
-// staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier)
-constexpr int RS_BAR2  = (RS_TOTAL + 127) / 128 * 128;
-constexpr int RS_L0    = RS_BAR2 + 128;
+constexpr int RE_LAUNCH = RE_TOTAL + PERF_RS_PAD;
+// experiment (PERF_FLAG_L0_SMEM, eval layout): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared
+// memory, staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier)
+constexpr int RE_BAR2  = (RE_TOTAL + 127) / 128 * 128;
+constexpr int RE_L0    = RE_BAR2 + 128;
 constexpr int L0_BYTES = 4096 * 8;
-constexpr int RS_TOTAL_L0 = RS_L0 + L0_BYTES;
+constexpr int RE_TOTAL_L0 = RE_L0 + L0_BYTES;
 
 // Output-layer weights of both networks as fp32 in the CONSTANT bank: [0,64) density row, [64,256) the three colour
 // rows.  The 64 * n_out FMAs per sample of the output layers then take their weight operand straight from c[bank][imm]
@@ -93,14 +115,15 @@ constexpr int RS_TOTAL_L0 = RS_L0 + L0_BYTES;
 // parameter vectors by weights_prepare_kernel, stream-ordered in front of every render launch (graph-capturable).
 // One slot per device: renders of DIFFERENT fields on the same device must not overlap in time (different streams).
 __constant__ float c_wout[4 * HID];
-// The three hidden-layer matrices as ready-made wgmma operand images (no-swizzle K-major canonical layout, mlp_tc.cuh), 16 KB:
-// every persistent CTA stages them with ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier) instead of 1024
-// 16-byte LDG + STS per CTA.  Written by the same preparation kernel, same single-slot rule as c_wout.
-__device__ uint4 g_wimg[W_IMG_BYTES / 16];
+// The three hidden-layer matrices as ready-made wgmma operand images (no-swizzle K-major canonical layout, mlp_tc.cuh), 16 KB,
+// followed by the two output layers as N = 8 operand images (2 x 1 KB, read by the eval kernels only): every persistent CTA
+// stages them with ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier) instead of 1024+ 16-byte LDG + STS per
+// CTA.  Written by the same preparation kernel, same single-slot rule as c_wout.
+__device__ uint4 g_wimg[W_IMG_ALL / 16];
 
 __global__ void __launch_bounds__(1024) weights_prepare_kernel(const __half* __restrict__ geo_w, const __half* __restrict__ app_w, float* __restrict__ c_dst)
 {
-    const int c = threadIdx.x;                       // 1024 threads = 1024 16-byte chunks of the images
+    const int c = threadIdx.x;                       // 1024 threads = 1024 16-byte chunks of the hidden images
     if (c < 4 * HID) c_dst[c] = __half2float(c < HID ? geo_w[HID * 32 + c] : app_w[HID * 32 + HID * HID + (c - HID)]);
     const __half* src; int K, cc;
     if (c < 256)      { src = geo_w;            K = 32; cc = c; }
@@ -108,17 +131,25 @@ __global__ void __launch_bounds__(1024) weights_prepare_kernel(const __half* __r
     else              { src = app_w + HID * 32; K = 64; cc = c - 512; }
     const int n = cc % HID, kg = cc / HID;           // image chunk (kg * 64 + n) <- row n, columns [8 kg, 8 kg + 8)
     g_wimg[c] = *reinterpret_cast<const uint4*>(src + (size_t)n * K + kg * 8);
+    if (c < 2 * WO_BYTES / 16) {                     // output images: chunk (kg * 8 + n) <- output row n, columns [8 kg, 8 kg + 8)
+        const int app = c >= WO_BYTES / 16, co = c % (WO_BYTES / 16), no = co % 8, kgo = co / 8;
+        const __half* wout = app ? app_w + HID * 32 + HID * HID : geo_w + HID * 32;      // [16 (padded), 64]
+        g_wimg[W_IMG_BYTES / 16 + c] = no < (app ? 3 : 1) ? *reinterpret_cast<const uint4*>(wout + no * HID + kgo * 8) : make_uint4(0, 0, 0, 0);
+    }
 }
 
-// all threads of the CTA: weight images global -> shared memory by one bulk copy; returns when they have landed
+// all threads of the CTA: weight images global -> shared memory by one bulk copy; returns when they have landed.
+// EVAL: the eval layout (RE_*, all five images); otherwise RS_* and the three hidden-layer images.
+template <bool EVAL>
 __device__ __forceinline__ void stage_weights_bulk(uint8_t* smem, int tid)
 {
-    uint64_t* barw = reinterpret_cast<uint64_t*>(smem + RS_BARW);
+    constexpr int bytes = EVAL ? W_IMG_ALL : W_IMG_BYTES;
+    uint64_t* barw = reinterpret_cast<uint64_t*>(smem + (EVAL ? RE_BARW : RS_BARW));
     if (tid == 0) {
         mbar_init(barw, 1); fence_mbar_init();
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(barw)), "r"(W_IMG_BYTES) : "memory");
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(barw)), "r"(bytes) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     :: "r"(smem_u32(smem + RS_W1G)), "l"(reinterpret_cast<const void*>(g_wimg)), "r"(W_IMG_BYTES), "r"(smem_u32(barw)) : "memory");
+                     :: "r"(smem_u32(smem + (EVAL ? RE_W1G : RS_W1G))), "l"(reinterpret_cast<const void*>(g_wimg)), "r"(bytes), "r"(smem_u32(barw)) : "memory");
     }
     __syncthreads();                                 // the barrier is initialised before anyone polls it
     mbar_wait(barw, 0);
@@ -222,7 +253,7 @@ static_assert(PATCH_WW * PATCH_WH == 32 && PATCH_WX * PATCH_WY == 4, "a warp is 
 
 struct RenderSmem {
     uint8_t *sA, *sAg, *sAa, *sH, *sW1g, *sW1a, *sW2a;
-    float *sWoutG, *sWoutA;
+    uint8_t *sWog, *sWoa;   // output-layer operand images (eval layout), or null
     const uint2* l0;        // level 0 of the packed table in shared memory, or null
 };
 
@@ -264,10 +295,10 @@ __device__ __forceinline__ uint4 ldg_cell(const uint4* p)
     return v;
 }
 
-// Levels [4q, 4q+4) of both fields -> one 16-byte k-group of each feature tile.
+// Levels [4q, 4q+4) of both fields -> one 16-byte k-group of row `row` of each feature tile.
 // KIND 0: generic addressing, 1: dense (fast), 2: hashed power-of-two (fast).
 template <int KIND, int SAVE, bool L0SMEM = false>
-__device__ __forceinline__ void encode_group(const RenderArgs& a, const RenderSmem& sm, int q, float x, float y, float z, int tid, uint64_t srow)
+__device__ __forceinline__ void encode_group(const RenderArgs& a, const RenderSmem& sm, int q, float x, float y, float z, int row, uint64_t srow)
 {
     uint32_t pg[4], pa[4];
 #pragma unroll
@@ -307,37 +338,128 @@ __device__ __forceinline__ void encode_group(const RenderArgs& a, const RenderSm
         for (int kk = 0; kk < 8; ++kk) { vg[kk] = v[kk].x; va[kk] = v[kk].y; }
         pg[ll] = blend8_half(w, vg); pa[ll] = blend8_half(w, va);
     }
-    *reinterpret_cast<uint4*>(sm.sAg + (q * TILE + tid) * 16) = make_uint4(pg[0], pg[1], pg[2], pg[3]);
-    *reinterpret_cast<uint4*>(sm.sAa + (q * TILE + tid) * 16) = make_uint4(pa[0], pa[1], pa[2], pa[3]);
+    *reinterpret_cast<uint4*>(sm.sAg + (q * TILE + row) * 16) = make_uint4(pg[0], pg[1], pg[2], pg[3]);
+    *reinterpret_cast<uint4*>(sm.sAa + (q * TILE + row) * 16) = make_uint4(pa[0], pa[1], pa[2], pa[3]);
     if constexpr (SAVE == 1) { if (srow != ~0ull) a.s_feat[srow * 4 + q] = make_uint4(pg[0], pg[1], pg[2], pg[3]); }
     if constexpr (SAVE == 2) { if (srow != ~0ull) a.s_feat[srow * 4 + q] = make_uint4(pa[0], pa[1], pa[2], pa[3]); }
 }
 
-// Encode + both MLPs for the CTA's current 128 samples (thread t = sample t at normalised
-// position (x,y,z)).  Contains 5 block-wide barriers; all 128 threads call it.
+// Both MLPs of the eval kernels with every hidden layer in registers (the FlashAttention-3 treatment of P: an m64nN fp32
+// accumulator fragment, ReLU-rounded pairwise to fp16, is the A-operand register fragment of the next m64nNk16 wgmma).
+// Thread (warp w, lane l) owns row eval_row() = 64 (l / 16) + 16 w + l % 16 of the feature tiles: M = 64 half l / 16, and
+// inside it rows [16w, 16w + 16) -- warp w's own slice of every fragment.  Per half h:
+//   layer 1 of both nets, A = feature tile, B = W1 image            -> relu_frag -> hg, ha
+//   colour layer 2 (A = ha, B = W2), density output (N = 8, A = hg)  -> relu_frag -> h2
+//   colour output (N = 8, A = h2)
+// Column c of in-warp row i of a half's N = 8 output is in lane 4 (i % 8) + c / 2, register 2 (i / 8) + c % 2, so every
+// output of the row a thread owns is in a lane of its own warp: 16 shuffles, no barrier.  Returns the fp32 pre-activations.
+// Shared memory is only read.  Before: the feature tiles are written, fenced for the async proxy and behind a barrier.  The
+// barrier after the last layer-1 wgmma has completed lets the caller write the next tile.
+__device__ __forceinline__ int eval_row(int tid) { return 64 * ((tid & 31) >> 4) + 16 * (tid >> 5) + (tid & 15); }
+
+__device__ __forceinline__ void eval_mlp_regs(const RenderSmem& sm, int lane, float& lg, float& lr, float& lgr, float& lb)
+{
+    float os[2][4], oc[2][4];                               // N = 8 output fragments of both halves
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        uint32_t hg[16], ha[16];
+        {
+            float dg[32], da[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { dg[i] = 0.f; da[i] = 0.f; }
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks)
+                wgmma_n64<0, 0>(dg, gmma_desc(smem_u32(sm.sAg) + h * 64 * 16 + ks * 2 * A_LBO, A_LBO, X_SBO),
+                                gmma_desc(smem_u32(sm.sW1g) + ks * 2 * W_LBO, W_LBO, X_SBO), ks > 0 ? 1u : 0u);
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks)
+                wgmma_n64<0, 0>(da, gmma_desc(smem_u32(sm.sAa) + h * 64 * 16 + ks * 2 * A_LBO, A_LBO, X_SBO),
+                                gmma_desc(smem_u32(sm.sW1a) + ks * 2 * W_LBO, W_LBO, X_SBO), ks > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait();
+            relu_frag(dg, hg);
+            relu_frag(da, ha);
+        }
+        if (h == 1) __syncthreads();                        // no warp reads the feature tiles any more
+        float d2[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d2[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { os[h][i] = 0.f; oc[h][i] = 0.f; }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+            wgmma_n64_ra(d2, ha + 4 * ks, gmma_desc(smem_u32(sm.sW2a) + ks * 2 * W_LBO, W_LBO, X_SBO), ks > 0 ? 1u : 0u);
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)                      // N = 8: one 8-row group, SBO unused
+            wgmma_n8_ra(os[h], hg + 4 * ks, gmma_desc(smem_u32(sm.sWog) + ks * 2 * WO_LBO, WO_LBO, X_SBO), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait();
+        uint32_t h2[16];
+        relu_frag(d2, h2);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+            wgmma_n8_ra(oc[h], h2 + 4 * ks, gmma_desc(smem_u32(sm.sWoa) + ks * 2 * WO_LBO, WO_LBO, X_SBO), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait();
+    }
+    // lane l wants column c of row l % 16 of half l / 16: register 2 ((l / 8) % 2) + c % 2 of half l / 16 in lane 4 (l % 8) + c / 2
+    const int src = 4 * (lane & 7);
+    const bool hi = (lane & 8) != 0, h1 = (lane & 16) != 0;
+    auto fetch = [&](const float (&o)[2][4], int c, int from) {
+        const float v0 = __shfl_sync(0xffffffffu, o[0][c], from), v1 = __shfl_sync(0xffffffffu, o[0][2 + c], from);
+        const float v2 = __shfl_sync(0xffffffffu, o[1][c], from), v3 = __shfl_sync(0xffffffffu, o[1][2 + c], from);
+        return h1 ? (hi ? v3 : v2) : (hi ? v1 : v0);
+    };
+    lg = fetch(os, 0, src);
+    lr = fetch(oc, 0, src); lgr = fetch(oc, 1, src); lb = fetch(oc, 0, src + 1);
+}
+
+// Encode + both MLPs for the CTA's current 128 samples (thread t = one sample at normalised position (x,y,z)); all
+// 128 threads call it.
+// EVAL (eval kernels: SIMT = false, SAVE = 0, eval shared-memory layout): hidden layers in registers (eval_mlp_regs), two
+// block-wide barriers.  Otherwise thread t owns row t of the tiles, every layer goes through shared memory and the output
+// layers run on CUDA cores (out_dots_const); 5 block-wide barriers.
 // NDENSE >= 0: specialised addressing (level_corners_fast; first NDENSE levels dense, rest hashed
 // power-of-two) -- branch-free and ~1/3 smaller code; NDENSE < 0: generic addressing.
 // SAVE 1 / 2: also write the fp16 features and hidden activations of the density / colour network
 // to row `srow` of the training buffers (srow == ~0: masked-out thread).
 // Shared-memory hazards across calls: every cross-row access (the layer MMAs and their fragment stores) sits between
 // barriers; everything else a thread touches is its own row.
-template <bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false>
+template <bool SIMT, int NDENSE, int SAVE, bool EVAL, bool L0SMEM = false>
 __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSmem& sm, float x, float y, float z, bool selector,
                                             int tid, float& sigma, float& cr, float& cg, float& cb, uint64_t srow = ~0ull)
 {
+    static_assert(!EVAL || (!SIMT && SAVE == 0), "the register MLP has no SIMT twin and no saves");
+    static_assert(!L0SMEM || EVAL, "level 0 in shared memory: eval layout only");
     uint8_t* const sA = sm.sA; uint8_t* const sAg = sm.sAg; uint8_t* const sAa = sm.sAa; uint8_t* const sH = sm.sH;
     uint8_t* const sW1g = sm.sW1g; uint8_t* const sW1a = sm.sW1a; uint8_t* const sW2a = sm.sW2a;
+    const int row = EVAL ? eval_row(tid) : tid;
     if (NDENSE >= 0 && !selector) { x = 0.5f; y = 0.5f; z = 0.5f; }   // masked sample: any in-box address will do
     // ---- encode both fields: 16 levels x 8 corners, one 8-byte gather per corner
     if constexpr (NDENSE == 4) {
         // dense group unrolled; the three hashed groups share ONE copy of the code (the fully
         // unrolled body stalled on instruction fetch)
-        encode_group<1, SAVE, L0SMEM>(a, sm, 0, x, y, z, tid, srow);
+        encode_group<1, SAVE, L0SMEM>(a, sm, 0, x, y, z, row, srow);
 #pragma unroll 1
-        for (int q = 1; q < 4; ++q) encode_group<2, SAVE>(a, sm, q, x, y, z, tid, srow);
+        for (int q = 1; q < 4; ++q) encode_group<2, SAVE>(a, sm, q, x, y, z, row, srow);
     } else {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) encode_group<0, SAVE>(a, sm, q, x, y, z, tid, srow);
+        for (int q = 0; q < 4; ++q) encode_group<0, SAVE>(a, sm, q, x, y, z, row, srow);
+    }
+
+    if constexpr (EVAL) {
+        fence_proxy_async();                                  // the feature tiles are the operand of layer 1
+        __syncthreads();
+        float lg, lr, lgr, lb;
+        eval_mlp_regs(sm, tid & 31, lg, lr, lgr, lb);
+        sigma = selector ? expf(finish_output(lg, 0)) : 0.f;  // ngp_nerf.py:141-150
+        cr = selector ? finish_output(lr, 1) : 0.f;           // ngp_nerf.py:156-161
+        cg = selector ? finish_output(lgr, 1) : 0.f;
+        cb = selector ? finish_output(lb, 1) : 0.f;
+        return;
     }
 
     // ---- layer 1 of both nets: density hidden -> H, colour hidden 1 -> A (over the feature tiles)
@@ -392,15 +514,13 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
     uint8_t* sW1g = smem + RS_W1G;
     uint8_t* sW1a = smem + RS_W1A;
     uint8_t* sW2a = smem + RS_W2A;
-    float*   sWoutG = reinterpret_cast<float*>(smem + RS_WOUT);
-    float*   sWoutA = sWoutG + HID;
     float*   sTails = reinterpret_cast<float*>(smem + RS_TAILS);
     float*   sCarry = reinterpret_cast<float*>(smem + RS_CARRY);
 
     const int tid = threadIdx.x;
-    const RenderSmem sm = {sA, sAg, sAa, sH, sW1g, sW1a, sW2a, sWoutG, sWoutA, nullptr};
+    const RenderSmem sm = {sA, sAg, sAa, sH, sW1g, sW1a, sW2a, nullptr, nullptr, nullptr};
 
-    stage_weights_bulk(smem, tid);                   // W1 density | W1 colour | W2 colour operand images, one bulk copy
+    stage_weights_bulk<false>(smem, tid);            // W1 density | W1 colour | W2 colour operand images, one bulk copy
 
     const uint32_t S = a.S;
     const float step = __fdiv_rn(__fsub_rn(a.far, a.near), (float)S);
@@ -450,7 +570,7 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
             const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
 
             float sigma, cr, cg, cb;
-            eval_fields<SIMT, -1>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb);
+            eval_fields<SIMT, -1, 0, false>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb);
 
             // ---- composite (nerf_renderer.py:170-183; oracle/composite.py)
             const float dt = __fsub_rn(te, ts);
@@ -498,26 +618,24 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
 template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false>
 __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(const __grid_constant__ RenderArgs a)
 {
+    constexpr bool EVAL = !SIMT && SAVE == 0;        // hidden layers in registers, eval shared-memory layout (RE_*)
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sA   = smem + RS_A;
-    uint8_t* sW1g = smem + RS_W1G;
-    uint8_t* sW1a = smem + RS_W1A;
-    uint8_t* sW2a = smem + RS_W2A;
-    float*   sWoutG = reinterpret_cast<float*>(smem + RS_WOUT);
-    float*   sWoutA = sWoutG + HID;
+    uint8_t* sA   = smem + (EVAL ? RE_A : RS_A);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const RenderSmem sm = {sA, sA, sA + A32_BYTES, smem + RS_H, sW1g, sW1a, sW2a, sWoutG, sWoutA,
-                           L0SMEM ? reinterpret_cast<const uint2*>(smem + RS_L0) : nullptr};
+    const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
+                                            smem + RE_WOA, L0SMEM ? reinterpret_cast<const uint2*>(smem + RE_L0) : nullptr}
+                               : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
+                                            nullptr, nullptr};
 
-    stage_weights_bulk(smem, tid);                   // W1 density | W1 colour | W2 colour operand images, one bulk copy
+    stage_weights_bulk<EVAL>(smem, tid);             // the weight operand images, one bulk copy
     if constexpr (L0SMEM) {
-        uint64_t* bar2 = reinterpret_cast<uint64_t*>(smem + RS_BAR2);
+        uint64_t* bar2 = reinterpret_cast<uint64_t*>(smem + RE_BAR2);
         if (tid == 0) {
             mbar_init(bar2, 1); fence_mbar_init();
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar2)), "r"(L0_BYTES) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"(smem_u32(smem + RS_L0)), "l"(a.table), "r"(L0_BYTES), "r"(smem_u32(bar2)) : "memory");
+                         :: "r"(smem_u32(smem + RE_L0)), "l"(a.table), "r"(L0_BYTES), "r"(smem_u32(bar2)) : "memory");
         }
         __syncthreads();                                   // the barrier is initialised before anyone polls it
         mbar_wait(bar2, 0);
@@ -591,7 +709,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             my_count = 0;
             if (valid) { pk_base = a.pk_offsets[ray]; my_count = (uint32_t)(a.pk_offsets[ray + 1] - pk_base); }
             const uint32_t wmax = __reduce_max_sync(0xffffffffu, my_count);
-            uint32_t* s_max = reinterpret_cast<uint32_t*>(smem + RS_TAILS);
+            uint32_t* s_max = reinterpret_cast<uint32_t*>(smem + (EVAL ? RE_MAX : RS_TAILS));
             __syncthreads();                                  // previous tile's readers are done
             if (lane == 0) s_max[warp] = wmax;
             __syncthreads();
@@ -619,7 +737,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
 
             float sigma, cr, cg, cb;
             const uint64_t srow = (SAVE != 0 && valid) ? (uint64_t)k * a.R + ray : ~0ull;
-            eval_fields<SIMT, NDENSE, SAVE, L0SMEM>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow);
+            eval_fields<SIMT, NDENSE, SAVE, EVAL, L0SMEM>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow);
 
             const float dt = __fsub_rn(te, ts);
             const float sd = sigma * dt;
@@ -712,15 +830,15 @@ struct PackedFieldArgs {
 template <int NDENSE, int SAVE>
 __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_constant__ RenderArgs a, const PackedFieldArgs p)
 {
+    constexpr bool EVAL = SAVE == 0;                 // hidden layers in registers, eval shared-memory layout (RE_*)
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sA   = smem + RS_A;
-    uint8_t* sW1g = smem + RS_W1G;
-    uint8_t* sW1a = smem + RS_W1A;
-    uint8_t* sW2a = smem + RS_W2A;
-    float*   sWoutG = reinterpret_cast<float*>(smem + RS_WOUT);
+    uint8_t* sA   = smem + (EVAL ? RE_A : RS_A);
     const int tid = threadIdx.x;
-    const RenderSmem sm = {sA, sA, sA + A32_BYTES, smem + RS_H, sW1g, sW1a, sW2a, sWoutG, sWoutG + HID, nullptr};
-    stage_weights_bulk(smem, tid);                   // W1 density | W1 colour | W2 colour operand images, one bulk copy
+    const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
+                                            smem + RE_WOA, nullptr}
+                               : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
+                                            nullptr, nullptr};
+    stage_weights_bulk<EVAL>(smem, tid);             // the weight operand images, one bulk copy
     uint64_t N = p.N;
     if (p.n_dev) { const int64_t nd = *p.n_dev; N = nd < 0 ? 0 : ((uint64_t)nd < N ? (uint64_t)nd : N); }      // graph-replayable count
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
@@ -741,7 +859,7 @@ __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_con
         }
         const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
         float sigma, cr, cg, cb;
-        eval_fields<false, NDENSE, SAVE>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull);
+        eval_fields<false, NDENSE, SAVE, EVAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull);
         if (valid) {
             p.sigma[n] = sigma;
             const __half2 c01 = __floats2half2_rn(cr, cg), c2 = __floats2half2_rn(cb, 0.f);
@@ -770,6 +888,25 @@ static void set_div_mode(RenderArgs& a)
 }
 
 static uint32_t gcd_u32(uint32_t a, uint32_t b) { while (b) { uint32_t t = a % b; a = b; b = t; } return a; }
+
+// Dynamic shared memory of a field kernel and its shared-memory carveout: the smallest that holds `ctas` resident CTAs (the
+// driver rounds the percentage up to the next size the SM supports), so that the rest of the SM's unified L1 / shared
+// memory stays L1 for the table gathers.  Not left to the driver's default: the eval layout (4 x 35 KB) fits the 164 KB
+// carveout, which leaves 92 KB of L1 where the 228 KB one leaves 28 KB.
+template <typename K>
+static int set_smem(K k, int bytes, int ctas)
+{
+    int dev = 0, max_smem = 0, reserved = 0;
+    PERF_CUDA(cudaGetDevice(&dev));
+    PERF_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    PERF_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+    const long long need = (long long)ctas * (bytes + reserved);
+    const long long pct_up = (100 * need + max_smem - 1) / max_smem;
+    const int pct = pct_up < 100 ? (int)pct_up : 100;
+    PERF_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    PERF_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    return PERF_OK;
+}
 
 static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano, cudaStream_t stream, int save = 0)
 {
@@ -815,37 +952,37 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         a.tile_mul = m % (uint32_t)n_work;
     }
     rc = prepare_weights(a, stream); if (rc) return rc;     // constant-bank output weights + operand images (c_wout, g_wimg)
-#define PERF_RENDER_LAUNCH(...) do { \
+    // BYTES: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RS_LAUNCH for the others
+#define PERF_RENDER_LAUNCH(BYTES, ...) do { \
         auto k = __VA_ARGS__; \
         static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
-        if (attr_dev != dev_) { PERF_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_LAUNCH)); \
-            attr_dev = dev_; } \
-        k<<<grid, TILE, RS_LAUNCH, stream>>>(a); } while (0)
+        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
+        k<<<grid, TILE, BYTES, stream>>>(a); } while (0)
     const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;   // PeRF's grid: 4 dense + 12 hashed levels
     if (save != 0) {
         PERF_CHECK_SUP(!pano && !simt && !scan, "training forward runs on the ray-marching tensor-core kernel only");
-        if (fast) { if (save == 1) PERF_RENDER_LAUNCH(render_march_kernel<false, false, 4, 1>); else PERF_RENDER_LAUNCH(render_march_kernel<false, false, 4, 2>); }
-        else      { if (save == 1) PERF_RENDER_LAUNCH(render_march_kernel<false, false, -1, 1>); else PERF_RENDER_LAUNCH(render_march_kernel<false, false, -1, 2>); }
+        if (fast) { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 2>); }
+        else      { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 2>); }
     } else if (scan) {
-        if (pano) { if (simt) PERF_RENDER_LAUNCH(render_kernel<true, true>); else PERF_RENDER_LAUNCH(render_kernel<true, false>); }
-        else      { if (simt) PERF_RENDER_LAUNCH(render_kernel<false, true>); else PERF_RENDER_LAUNCH(render_kernel<false, false>); }
+        if (pano) { if (simt) PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<true, true>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<true, false>); }
+        else      { if (simt) PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<false, true>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<false, false>); }
     } else if (simt) {
-        if (pano) PERF_RENDER_LAUNCH(render_march_kernel<true, true, -1>); else PERF_RENDER_LAUNCH(render_march_kernel<false, true, -1>);
+        if (pano) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<true, true, -1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, true, -1>);
     } else if (fast && pano && (args->flags & PERF_FLAG_L0_SMEM)) {
         auto k = render_march_kernel<true, false, 4, 0, true>;           // experiment: level 0 in shared memory (2 CTAs/SM)
         static thread_local int attr_dev0 = -1, per_sm0 = 1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_));
         if (attr_dev0 != dev_) {
-            PERF_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_TOTAL_L0));
-            PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm0, k, TILE, RS_TOTAL_L0));
+            rc = set_smem(k, RE_TOTAL_L0, 2); if (rc) return rc;
+            PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm0, k, TILE, RE_TOTAL_L0));
             if (per_sm0 < 1) per_sm0 = 1;
             attr_dev0 = dev_;
         }
         const uint64_t slots0 = (uint64_t)num_sms() * (uint64_t)per_sm0;
-        k<<<(unsigned)(n_work < slots0 ? n_work : slots0), TILE, RS_TOTAL_L0, stream>>>(a);
+        k<<<(unsigned)(n_work < slots0 ? n_work : slots0), TILE, RE_TOTAL_L0, stream>>>(a);
     } else if (fast) {
-        if (pano) PERF_RENDER_LAUNCH(render_march_kernel<true, false, 4>); else PERF_RENDER_LAUNCH(render_march_kernel<false, false, 4>);
+        if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<true, false, 4>); else PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<false, false, 4>);
     } else {
-        if (pano) PERF_RENDER_LAUNCH(render_march_kernel<true, false, -1>); else PERF_RENDER_LAUNCH(render_march_kernel<false, false, -1>);
+        if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<true, false, -1>); else PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<false, false, -1>);
     }
 #undef PERF_RENDER_LAUNCH
     PERF_LAUNCH_CHECK();
@@ -937,19 +1074,20 @@ int perf_fields_packed(const perf_render_args* args, const float* d_rays_o, cons
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
     const unsigned grid = (unsigned)(n_tiles < (uint64_t)num_sms() * 4 ? n_tiles : (uint64_t)num_sms() * 4);
     const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
-#define PERF_PACKED_LAUNCH(...) do { \
+    // BYTES: RE_TOTAL for the eval kernels (phase 0), RS_TOTAL for the saving ones
+#define PERF_PACKED_LAUNCH(BYTES, ...) do { \
         auto k = __VA_ARGS__; \
         static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
-        if (attr_dev != dev_) { PERF_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_TOTAL)); attr_dev = dev_; } \
-        k<<<grid, TILE, RS_TOTAL, st>>>(a, p); } while (0)
+        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
+        k<<<grid, TILE, BYTES, st>>>(a, p); } while (0)
     if (fast) {
-        if (phase == 0) PERF_PACKED_LAUNCH(packed_fields_kernel<4, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(packed_fields_kernel<4, 1>);
-        else PERF_PACKED_LAUNCH(packed_fields_kernel<4, 2>);
+        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<4, 0>);
+        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 1>);
+        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 2>);
     } else {
-        if (phase == 0) PERF_PACKED_LAUNCH(packed_fields_kernel<-1, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(packed_fields_kernel<-1, 1>);
-        else PERF_PACKED_LAUNCH(packed_fields_kernel<-1, 2>);
+        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<-1, 0>);
+        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 1>);
+        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 2>);
     }
 #undef PERF_PACKED_LAUNCH
     PERF_LAUNCH_CHECK();
