@@ -207,6 +207,29 @@ int perf_render_packed(const perf_render_args* args, const float* d_rays_o, cons
 int perf_render_pano(const perf_render_args* args, const float* h_pose, int H, int W,
                      int row0, int rows, void* stream);
 
+/* ---- surface normals: the three renders above (and perf_fields_packed) with a fourth output.
+ * Definition, per sample at normalised position x01 (the renderer's own position, selector and fp16 features):
+ *   h = W1 f (the density net's layer-1 pre-activation, fp32), m_j = [h_j > 0],
+ *   g = W1^T (m . w_out) (fp16 weights as fp32; the forward's fp16 roundings count as identity),
+ *   d raw / d x01_d = sum_levels sum_features g * scale * A_d (Linear interpolation; perf_hashgrid_bwd_input's arithmetic
+ *   on the fp16 geo entries), raw = the density logit BEFORE trunc_exp (same direction: sigma = exp(raw)),
+ *   grad_d = (d raw / d x01_d) / (aabb max_d - min_d),  n = -grad / |grad|;  n = 0 when the selector is false or |grad| = 0.
+ * Per ray: d_normal [R,3] fp32 = sum_i w_i n_i with the weights that produce distance / opacity -- no background term, no
+ * normalisation (|normal| <= opacity; normalise for display).  rgb / distance / opacity are the plain entry points' outputs.
+ * Eval mode on the ray-marching wgmma kernel only: PERF_FLAG_SIMT_MLP, PERF_FLAG_SCAN_KERNEL, PERF_FLAG_L0_SMEM and
+ * PERF_FLAG_TRAINING return PERF_EUNSUPPORTED. */
+int perf_render_pano_normals(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows,
+                             float* d_normal, void* stream);
+/* Explicit rays (args->image_width > 0: a row-major image, pixel-patch tiling as perf_render_rays). */
+int perf_render_rays_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R,
+                             float* d_normal, void* stream);
+/* perf_fields_packed, phase 0 (no saves), plus the sample normal n (definition above) d_normal [N,3] of every packed sample.
+ * The occupancy render's ray normal is then perf_composite_packed_fwd (d_weights, with its early_stop_eps cut) followed by
+ * perf_accumulate_along_rays(d_weights, d_normal, D = 3). */
+int perf_fields_packed_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, const int64_t* d_ray_indices,
+                               const float* d_t_starts, const float* d_t_ends, uint64_t N, const int64_t* d_n_dev /* nullable */,
+                               float* d_sigma, void* d_rgb_half4, float* d_x01, float* d_normal, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

@@ -12,6 +12,7 @@
 //   gen_pano_rays                       utils/camera_utils.py:229-234
 // Arithmetic contract: oracle/render.py::render_rays(mixed=True).
 #include "mlp_tc.cuh"
+#include "grid_grad.cuh"
 
 namespace perf {
 
@@ -58,7 +59,10 @@ struct RenderArgs {
     // results are combined with the transmittance product rule.  Fills the GPU for small ray batches
     // (an 8192-ray training batch is only 64 tiles of 128 rays, but 512 tiles of 16 rays x 8 segments).
     uint32_t      seg;          // power of two, divides S and 128; 1 = off
-    float*        s_toff;       // [seg * R] transmittance at the start of each segment (SAVE, seg > 1)
+    union {
+        float*    s_toff;       // [seg * R] transmittance at the start of each segment (SAVE, seg > 1)
+        float*    normal;       // [R,3] sum_i w_i n_i per ray (NORMAL kernels: eval, seg == 1)
+    };
 };
 
 // Shared memory of the kernels that round-trip the hidden layers through shared memory: the training forward (SAVE = 1/2),
@@ -94,6 +98,12 @@ constexpr int W_IMG_ALL = W_IMG_BYTES + 2 * WO_BYTES;                // 18 KB: t
 static_assert(RE_W1A == RE_W1G + W32_BYTES && RE_W2A == RE_W1A + W32_BYTES && RE_WOG == RE_W1G + W_IMG_BYTES &&
               RE_WOA == RE_WOG + WO_BYTES, "the five weight images are one contiguous block");
 static_assert(4 * (RE_TOTAL + 1024) <= 164 * 1024, "4 eval CTAs (+1 KB reserved each) fit the 164 KB shared-memory carveout");
+// The normals kernels (NORMAL) append per thread the sample position and the ray's running sum w n: the layer-1 peak of
+// the MLP leaves no register for them (the eval march kernel uses all 128 without them).
+constexpr int RE_XYZ   = (RE_TOTAL + 15) / 16 * 16;    // float4 [128]: x01, selector
+constexpr int RE_NACC  = RE_XYZ + TILE * 16;            // float4 [128]: sum w n of the thread's ray (march kernel)
+constexpr int RE_TOTAL_N = RE_NACC + TILE * 16;
+static_assert(4 * (RE_TOTAL_N + 1024) <= 164 * 1024, "4 normals CTAs fit the 164 KB shared-memory carveout");
 // measurement hook (tools/ab_lib.py): extra, unused dynamic shared memory per CTA of the march kernels, i.e. what
 // more shared memory would cost in L1 capacity
 #ifndef PERF_RS_PAD
@@ -101,6 +111,7 @@ static_assert(4 * (RE_TOTAL + 1024) <= 164 * 1024, "4 eval CTAs (+1 KB reserved 
 #endif
 constexpr int RS_LAUNCH = RS_TOTAL + PERF_RS_PAD;
 constexpr int RE_LAUNCH = RE_TOTAL + PERF_RS_PAD;
+constexpr int RE_LAUNCH_N = RE_TOTAL_N + PERF_RS_PAD;
 // experiment (PERF_FLAG_L0_SMEM, eval layout): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared
 // memory, staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier)
 constexpr int RE_BAR2  = (RE_TOTAL + 127) / 128 * 128;
@@ -255,6 +266,7 @@ struct RenderSmem {
     uint8_t *sA, *sAg, *sAa, *sH, *sW1g, *sW1a, *sW2a;
     uint8_t *sWog, *sWoa;   // output-layer operand images (eval layout), or null
     const uint2* l0;        // level 0 of the packed table in shared memory, or null
+    float4* xyz;            // NORMAL kernels: [128] each thread's sample position + selector across the MLP, or null
 };
 
 // base + 8 * idx as ONE IMAD.WIDE.U32 (left to itself ptxas splits the 64-bit address into LEA + IADD3.X per corner)
@@ -417,6 +429,130 @@ __device__ __forceinline__ void eval_mlp_regs(const RenderSmem& sm, int lane, fl
     lr = fetch(oc, 0, src); lgr = fetch(oc, 1, src); lb = fetch(oc, 0, src + 1);
 }
 
+// ---- surface normals (NORMAL kernels): n = -grad(raw) / |grad(raw)| of the density logit raw = w_out . ReLU(W1 f(x))
+// Data gradient of the density net for the tile, g = W1^T (m . w_out) with m = [W1 f > 0] (the fp32 layer-1 accumulator;
+// the fp16 roundings of the forward count as identity): per M = 64 half one m64n32 wgmma, A = the masked output row in
+// registers (the relu_frag layout of the layer-1 fragment), B = the staged W1 image read MN-major (mlp_bwd.cu).  The fp32
+// result is staged into the feature tiles, idle since the last layer-1 wgmma: column chunk c (4 floats) of tile row r
+// goes where k-group c % 4 of row r of feature tile c / 4 lives, so a warp writes and reads only the slots of its own
+// rows (eval_row) -- no block barrier, and the next tile's encode overwrites nothing another warp still reads.
+__device__ __forceinline__ uint32_t g_slot(int row, int c) { return (uint32_t)((c >> 2) * A32_BYTES + (c & 3) * A_LBO + row * 16); }
+
+// Called after eval_mlp_regs, by all 128 threads.  The mask is the density layer 1 once more (the forward's wgmma on the
+// unchanged feature tile: the same fp32 accumulator), so that no register stays live across the forward for it.
+__device__ __forceinline__ void eval_density_g(const RenderSmem& sm, int tid)
+{
+    const int warp = tid >> 5, lane = tid & 31, q = lane & 3;
+    uint32_t gm[2];                                          // bit i of gm[h]: [dg[i] > 0] of half h's fragment
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float dg[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) dg[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks)
+            wgmma_n64<0, 0>(dg, gmma_desc(smem_u32(sm.sAg) + h * 64 * 16 + ks * 2 * A_LBO, A_LBO, X_SBO),
+                            gmma_desc(smem_u32(sm.sW1g) + ks * 2 * W_LBO, W_LBO, X_SBO), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait();
+        uint32_t m = 0;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) m |= (dg[i] > 0.f ? 1u : 0u) << i;
+        gm[h] = m;
+    }
+    __syncthreads();                                         // no warp reads the feature tiles any more: g may overwrite them
+    uint32_t wo[8];                                          // w_out columns 8j + 2q, +1 (fp16 pair; output image row 0)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) wo[j] = *reinterpret_cast<const uint32_t*>(sm.sWog + j * 128 + q * 4);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        uint32_t am[16];                                     // register i = accumulator pair (2i, 2i + 1): w_out pair i / 2
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+            am[i] = wo[i >> 1] & (((gm[h] >> (2 * i)) & 1u ? 0x0000FFFFu : 0u) | ((gm[h] >> (2 * i + 1)) & 1u ? 0xFFFF0000u : 0u));
+        float d[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)                       // K = the 64 hidden units; N = the 32 features
+            wgmma_n32_ra_tb(d, am + 4 * ks, gmma_desc(smem_u32(sm.sW1g) + ks * 256, 128, W_LBO), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait();
+        // d[4j + e]: row 64h + 16 warp + lane / 4 + 8 (e / 2), columns 8j + 2q + (e % 2) = chunk 2j + q / 2, float (2q) % 4 + e % 2
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; e += 2) {
+                const int row = 64 * h + 16 * warp + (lane >> 2) + 4 * e;
+                *reinterpret_cast<float2*>(sm.sA + g_slot(row, 2 * j + (q >> 1)) + (q & 1) * 8) = make_float2(d[4 * j + e], d[4 * j + e + 1]);
+            }
+    }
+    __syncwarp();
+}
+
+// One level of d raw / d x01 (grid_grad.cuh::level_input_grad, Linear on the fast paths): the corners are addressed as the
+// forward addresses them and only the geo half of each packed entry is used.  KIND as encode_group.
+template <int KIND>
+__device__ __forceinline__ void normal_level(const RenderArgs& a, int l, float x, float y, float z, float2 gl, float (&acc)[3])
+{
+    LevelFrame f;
+    float2 v[8];
+    if constexpr (KIND == 0) {
+        level_frame(a.lt, l, x, y, z, f);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = unpack_half2(__ldg(&a.table[f.idx[k]].x));
+    } else {
+        const float scale = a.lt.scale[l];
+        const float in[3] = {x, y, z};
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            const float pos = fmaf(scale, in[d], 0.5f);
+            f.s[d] = pos - floorf(pos); f.ds[d] = 1.f; f.dds[d] = 0.f;
+        }
+        f.scale = scale;
+        float w[8];
+        if constexpr (KIND == 1) {
+            const uint4* const cp = a.cells[l] + 4ull * level_cell_dense(a.lt, l, x, y, z, w);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint4 c2 = ldg_cell<PERF_L1_DENSE>(cp + j);
+                v[2 * j] = unpack_half2(c2.x); v[2 * j + 1] = unpack_half2(c2.z);
+            }
+        } else {
+            uint32_t idx[8];
+            level_corners_rel<true>(a.lt, l, x, y, z, idx, w);
+            const uint2* const tl = a.table + a.lt.offset[l];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = unpack_half2(__ldg(&entry_ptr(tl, idx[k])->x));
+        }
+    }
+    level_input_grad(f, v, gl, acc);
+}
+
+// This thread's sample normal (selector true): the 16 levels again with dL/dfeature = the staged row of g, then the world
+// gradient grad_d = (d raw / d x01_d) / aabb_ext_d and n = -grad / |grad| (0 when |grad| = 0).
+template <int NDENSE>
+__device__ __forceinline__ void sample_normal(const RenderArgs& a, const RenderSmem& sm, float x, float y, float z, int row, float (&n)[3])
+{
+    float acc[3] = {0.f, 0.f, 0.f};
+    const uint8_t* const g_row = sm.sA + g_slot(row, 0);
+    auto gl = [&](int l) { return *reinterpret_cast<const float2*>(g_row + g_slot(0, l >> 1) + (l & 1) * 8); };
+    if constexpr (NDENSE == 4) {
+#pragma unroll 1
+        for (int l = 0; l < 4; ++l) normal_level<1>(a, l, x, y, z, gl(l), acc);
+#pragma unroll 1
+        for (int l = 4; l < 16; ++l) normal_level<2>(a, l, x, y, z, gl(l), acc);
+    } else {
+#pragma unroll 1
+        for (int l = 0; l < 16; ++l) normal_level<0>(a, l, x, y, z, gl(l), acc);
+    }
+    const float gx = acc[0] / a.aabb_ext[0], gy = acc[1] / a.aabb_ext[1], gz = acc[2] / a.aabb_ext[2];
+    const float r = fmaxf(fabsf(gx), fmaxf(fabsf(gy), fabsf(gz))) > 0.f ? rnorm3df(gx, gy, gz) : 0.f;
+    n[0] = -gx * r; n[1] = -gy * r; n[2] = -gz * r;
+}
+
 // Encode + both MLPs for the CTA's current 128 samples (thread t = one sample at normalised position (x,y,z)); all
 // 128 threads call it.
 // EVAL (eval kernels: SIMT = false, SAVE = 0, eval shared-memory layout): hidden layers in registers (eval_mlp_regs), two
@@ -428,16 +564,20 @@ __device__ __forceinline__ void eval_mlp_regs(const RenderSmem& sm, int lane, fl
 // to row `srow` of the training buffers (srow == ~0: masked-out thread).
 // Shared-memory hazards across calls: every cross-row access (the layer MMAs and their fragment stores) sits between
 // barriers; everything else a thread touches is its own row.
-template <bool SIMT, int NDENSE, int SAVE, bool EVAL, bool L0SMEM = false>
+// NORMAL (eval layout only): also nrm[3] = the sample's surface normal (sample_normal; 0 for a masked-out sample).
+template <bool SIMT, int NDENSE, int SAVE, bool EVAL, bool L0SMEM = false, bool NORMAL = false>
 __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSmem& sm, float x, float y, float z, bool selector,
-                                            int tid, float& sigma, float& cr, float& cg, float& cb, uint64_t srow = ~0ull)
+                                            int tid, float& sigma, float& cr, float& cg, float& cb, uint64_t srow = ~0ull,
+                                            float* nrm = nullptr)
 {
     static_assert(!EVAL || (!SIMT && SAVE == 0), "the register MLP has no SIMT twin and no saves");
     static_assert(!L0SMEM || EVAL, "level 0 in shared memory: eval layout only");
+    static_assert(!NORMAL || (EVAL && !L0SMEM), "normals: eval layout without level 0 in shared memory");
     uint8_t* const sA = sm.sA; uint8_t* const sAg = sm.sAg; uint8_t* const sAa = sm.sAa; uint8_t* const sH = sm.sH;
     uint8_t* const sW1g = sm.sW1g; uint8_t* const sW1a = sm.sW1a; uint8_t* const sW2a = sm.sW2a;
     const int row = EVAL ? eval_row(tid) : tid;
     if (NDENSE >= 0 && !selector) { x = 0.5f; y = 0.5f; z = 0.5f; }   // masked sample: any in-box address will do
+    if constexpr (NORMAL) sm.xyz[tid] = make_float4(x, y, z, selector ? 1.f : 0.f);   // own slot: read back after the MLP
     // ---- encode both fields: 16 levels x 8 corners, one 8-byte gather per corner
     if constexpr (NDENSE == 4) {
         // dense group unrolled; the three hashed groups share ONE copy of the code (the fully
@@ -455,6 +595,14 @@ __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSme
         __syncthreads();
         float lg, lr, lgr, lb;
         eval_mlp_regs(sm, tid & 31, lg, lr, lgr, lb);
+        if constexpr (NORMAL) {
+            eval_density_g(sm, tid);
+            const float4 p = sm.xyz[tid];
+            float n[3] = {0.f, 0.f, 0.f};
+            if (p.w != 0.f) sample_normal<NDENSE>(a, sm, p.x, p.y, p.z, row, n);
+            __syncwarp();                                     // g is read: the next tile's encode may overwrite the slots
+            nrm[0] = n[0]; nrm[1] = n[1]; nrm[2] = n[2];
+        }
         sigma = selector ? expf(finish_output(lg, 0)) : 0.f;  // ngp_nerf.py:141-150
         cr = selector ? finish_output(lr, 1) : 0.f;           // ngp_nerf.py:156-161
         cg = selector ? finish_output(lgr, 1) : 0.f;
@@ -615,7 +763,8 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
 // per request at the coarse and middle levels) and a thread revisits the same cells from k to k+1
 // (temporal L1 reuse).  The composite is a per-thread running sum: no shuffles, no carries.
 // Transmittance uses the sequential exclusive sum, the order of the oracle's cumsum.
-template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false>
+// NORMAL: also a.normal[ray] = sum_i w_i n_i (eval layout, seg == 1).
+template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false, bool NORMAL = false>
 __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(const __grid_constant__ RenderArgs a)
 {
     constexpr bool EVAL = !SIMT && SAVE == 0;        // hidden layers in registers, eval shared-memory layout (RE_*)
@@ -624,7 +773,8 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
-                                            smem + RE_WOA, L0SMEM ? reinterpret_cast<const uint2*>(smem + RE_L0) : nullptr}
+                                            smem + RE_WOA, L0SMEM ? reinterpret_cast<const uint2*>(smem + RE_L0) : nullptr,
+                                            NORMAL ? reinterpret_cast<float4*>(smem + RE_XYZ) : nullptr}
                                : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
                                             nullptr, nullptr};
 
@@ -701,6 +851,8 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
         float sum_sd = 0.f;                                   // exclusive running sum of sigma*dt
         float acc_w = 0.f, acc_d = 0.f, acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;
         float dl_uni = 0.f, dl_bi = 0.f;                      // distortion loss pieces (SAVE only)
+        float4* const acc_n = reinterpret_cast<float4*>(smem + RE_NACC) + tid;     // sum w n (NORMAL only)
+        if constexpr (NORMAL) *acc_n = make_float4(0.f, 0.f, 0.f, 0.f);
         // packed mode: every thread walks ITS ray's samples; the tile iterates to the longest ray
         // (neighbouring rays cross the same occupied shells, so lengths inside a tile are similar)
         uint32_t n_iter = kps, my_count = S;
@@ -735,9 +887,9 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             const float z = div_uniform(__fsub_rn(pz, a.aabb_min[2]), a.aabb_ext[2], rext2, a.div_generic != 0u);
             const bool selector = live && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
 
-            float sigma, cr, cg, cb;
+            float sigma, cr, cg, cb, nrm[3];
             const uint64_t srow = (SAVE != 0 && valid) ? (uint64_t)k * a.R + ray : ~0ull;
-            eval_fields<SIMT, NDENSE, SAVE, EVAL, L0SMEM>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow);
+            eval_fields<SIMT, NDENSE, SAVE, EVAL, L0SMEM, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow, nrm);
 
             const float dt = __fsub_rn(te, ts);
             const float sd = sigma * dt;
@@ -759,6 +911,11 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             }
             acc_w += w; acc_d = fmaf(w, tsum * 0.5f, acc_d);
             acc_r = fmaf(w, cr, acc_r); acc_g = fmaf(w, cg, acc_g); acc_b = fmaf(w, cb, acc_b);
+            if constexpr (NORMAL) {
+                float4 an = *acc_n;
+                an.x = fmaf(w, nrm[0], an.x); an.y = fmaf(w, nrm[1], an.y); an.z = fmaf(w, nrm[2], an.z);
+                *acc_n = an;
+            }
             if constexpr (SIMT) __syncthreads();
         }
 
@@ -806,6 +963,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             a.rgb[3 * ray] = r; a.rgb[3 * ray + 1] = g; a.rgb[3 * ray + 2] = b;
             a.distance[ray] = dist;
             if (a.opacity) a.opacity[ray] = acc_w;
+            if constexpr (NORMAL) { const float4 an = *acc_n; a.normal[3 * ray] = an.x; a.normal[3 * ray + 1] = an.y; a.normal[3 * ray + 2] = an.z; }
         }
     }
 }
@@ -825,9 +983,10 @@ struct PackedFieldArgs {
     float*         sigma;         // [N]
     __half*        rgb;           // [N,4] fp16
     float*         x01;           // [N,3]
+    float*         normal;        // [N,3] sample normals (NORMAL kernels)
 };
 
-template <int NDENSE, int SAVE>
+template <int NDENSE, int SAVE, bool NORMAL = false>
 __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_constant__ RenderArgs a, const PackedFieldArgs p)
 {
     constexpr bool EVAL = SAVE == 0;                 // hidden layers in registers, eval shared-memory layout (RE_*)
@@ -835,7 +994,7 @@ __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_con
     uint8_t* sA   = smem + (EVAL ? RE_A : RS_A);
     const int tid = threadIdx.x;
     const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
-                                            smem + RE_WOA, nullptr}
+                                            smem + RE_WOA, nullptr, NORMAL ? reinterpret_cast<float4*>(smem + RE_XYZ) : nullptr}
                                : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
                                             nullptr, nullptr};
     stage_weights_bulk<EVAL>(smem, tid);             // the weight operand images, one bulk copy
@@ -858,10 +1017,11 @@ __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_con
             z = div_uniform(__fsub_rn(pz, a.aabb_min[2]), a.aabb_ext[2], rext2, a.div_generic != 0u);
         }
         const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
-        float sigma, cr, cg, cb;
-        eval_fields<false, NDENSE, SAVE, EVAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull);
+        float sigma, cr, cg, cb, nrm[3];
+        eval_fields<false, NDENSE, SAVE, EVAL, false, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull, nrm);
         if (valid) {
             p.sigma[n] = sigma;
+            if constexpr (NORMAL) { p.normal[3 * n] = nrm[0]; p.normal[3 * n + 1] = nrm[1]; p.normal[3 * n + 2] = nrm[2]; }
             const __half2 c01 = __floats2half2_rn(cr, cg), c2 = __floats2half2_rn(cb, 0.f);
             *reinterpret_cast<uint2*>(p.rgb + n * 4) = make_uint2(*reinterpret_cast<const uint32_t*>(&c01), *reinterpret_cast<const uint32_t*>(&c2));
             // masked-out samples: the in-box stand-in position the features were taken at (their gradient is zero)
@@ -908,7 +1068,8 @@ static int set_smem(K k, int bytes, int ctas)
     return PERF_OK;
 }
 
-static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano, cudaStream_t stream, int save = 0)
+// normals: a.normal is set (it shares its slot with a.s_toff, so only this flag selects the NORMAL kernels)
+static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano, cudaStream_t stream, int save = 0, bool normals = false)
 {
     PERF_CHECK_ARG(args->d_packed_table && args->d_geo_mlp_half && args->d_app_mlp_half, "NULL table / weights");
     PERF_CHECK_ARG(args->d_rgb && args->d_distance, "NULL output");
@@ -952,14 +1113,17 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         a.tile_mul = m % (uint32_t)n_work;
     }
     rc = prepare_weights(a, stream); if (rc) return rc;     // constant-bank output weights + operand images (c_wout, g_wimg)
-    // BYTES: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RS_LAUNCH for the others
+    // BYTES: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RE_LAUNCH_N for their normals twins, RS_LAUNCH for the others
 #define PERF_RENDER_LAUNCH(BYTES, ...) do { \
         auto k = __VA_ARGS__; \
         static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
         if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
         k<<<grid, TILE, BYTES, stream>>>(a); } while (0)
     const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;   // PeRF's grid: 4 dense + 12 hashed levels
-    if (save != 0) {
+    if (normals) {                                                // surface normals: eval march kernel only (the callers refuse the rest)
+        if (fast) { if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<true, false, 4, 0, false, true>); else PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<false, false, 4, 0, false, true>); }
+        else      { if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<true, false, -1, 0, false, true>); else PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<false, false, -1, 0, false, true>); }
+    } else if (save != 0) {
         PERF_CHECK_SUP(!pano && !simt && !scan, "training forward runs on the ray-marching tensor-core kernel only");
         if (fast) { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 2>); }
         else      { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 2>); }
@@ -985,6 +1149,58 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<true, false, -1>); else PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<false, false, -1>);
     }
 #undef PERF_RENDER_LAUNCH
+    PERF_LAUNCH_CHECK();
+    return PERF_OK;
+}
+
+// perf_fields_packed and perf_fields_packed_normals (d_normal != null: phase 0 only)
+static int fields_packed(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, const int64_t* d_ray_indices,
+                         const float* d_t_starts, const float* d_t_ends, uint64_t N, const int64_t* d_n_dev, int phase, float* d_sigma, void* d_rgb_half4,
+                         float* d_x01, void* d_feat, void* d_h1, void* d_h2, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && d_rays_o && d_rays_d && d_ray_indices && d_t_starts && d_t_ends && d_sigma && d_rgb_half4 && d_x01, "NULL pointer");
+    PERF_CHECK_ARG(phase == 0 || phase == PERF_PHASE_GEO || phase == PERF_PHASE_APP, "phase must be 0, PERF_PHASE_GEO or PERF_PHASE_APP");
+    PERF_CHECK_ARG(phase == 0 || (d_feat && d_h1 && (phase == PERF_PHASE_GEO || d_h2)), "NULL save buffer");
+    PERF_CHECK_ARG(args->d_packed_table && args->d_geo_mlp_half && args->d_app_mlp_half, "NULL table / weights");
+    PERF_CHECK_ARG(((uintptr_t)d_feat | (uintptr_t)d_h1 | (uintptr_t)d_h2) % 16 == 0 && (uintptr_t)d_rgb_half4 % 8 == 0, "misaligned buffer");
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    uint64_t n_entries = 0;
+    int rc = build_level_table(&args->grid, &a.lt, &n_entries); if (rc) return rc;
+    PERF_CHECK_SUP(args->grid.n_levels == 16, "fused field kernel needs n_levels == 16 (got %u)", args->grid.n_levels);
+    a.table = (const uint2*)args->d_packed_table;
+    PERF_CHECK_ARG((uintptr_t)args->d_packed_table % 16 == 0, "misaligned table");
+    const PackedLayout pl = packed_layout(a.lt, n_entries);
+    for (uint32_t l = 0; l < pl.n_cell_levels; ++l) a.cells[l] = reinterpret_cast<const uint4*>(a.table + pl.cell_start[l]);
+    a.geo_w = (const __half*)args->d_geo_mlp_half; a.app_w = (const __half*)args->d_app_mlp_half;
+    for (int i = 0; i < 3; ++i) { a.aabb_min[i] = args->aabb[i]; a.aabb_ext[i] = args->aabb[3 + i] - args->aabb[i]; }
+    set_div_mode(a);
+    a.rays_o = d_rays_o; a.rays_d = d_rays_d;
+    a.s_feat = (uint4*)d_feat; a.s_h1 = (uint4*)d_h1; a.s_h2 = (uint4*)d_h2;
+    if (N == 0) return PERF_OK;
+    PackedFieldArgs p = {d_ray_indices, d_t_starts, d_t_ends, N, d_n_dev, d_sigma, (__half*)d_rgb_half4, d_x01, d_normal};
+    cudaStream_t st = (cudaStream_t)stream;
+    rc = prepare_weights(a, st); if (rc) return rc;
+    const uint64_t n_tiles = (N + TILE - 1) / TILE;
+    const unsigned grid = (unsigned)(n_tiles < (uint64_t)num_sms() * 4 ? n_tiles : (uint64_t)num_sms() * 4);
+    const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
+    // BYTES: RE_TOTAL for the eval kernels (phase 0), RS_TOTAL for the saving ones
+#define PERF_PACKED_LAUNCH(BYTES, ...) do { \
+        auto k = __VA_ARGS__; \
+        static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
+        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
+        k<<<grid, TILE, BYTES, st>>>(a, p); } while (0)
+    if (p.normal != nullptr) {
+        if (fast) PERF_PACKED_LAUNCH(RE_TOTAL_N, packed_fields_kernel<4, 0, true>); else PERF_PACKED_LAUNCH(RE_TOTAL_N, packed_fields_kernel<-1, 0, true>);
+    } else if (fast) {
+        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<4, 0>);
+        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 1>);
+        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 2>);
+    } else {
+        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<-1, 0>);
+        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 1>);
+        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 2>);
+    }
+#undef PERF_PACKED_LAUNCH
     PERF_LAUNCH_CHECK();
     return PERF_OK;
 }
@@ -1045,53 +1261,13 @@ int perf_train_forward(const perf_render_args* args, const float* d_rays_o, cons
     return launch_render(&t, a, false, (cudaStream_t)stream, phase);
 }
 
+
 int perf_fields_packed(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, const int64_t* d_ray_indices,
                        const float* d_t_starts, const float* d_t_ends, uint64_t N, const int64_t* d_n_dev, int phase, float* d_sigma, void* d_rgb_half4,
                        float* d_x01, void* d_feat, void* d_h1, void* d_h2, void* stream)
 {
-    PERF_CHECK_ARG(args && d_rays_o && d_rays_d && d_ray_indices && d_t_starts && d_t_ends && d_sigma && d_rgb_half4 && d_x01, "NULL pointer");
-    PERF_CHECK_ARG(phase == 0 || phase == PERF_PHASE_GEO || phase == PERF_PHASE_APP, "phase must be 0, PERF_PHASE_GEO or PERF_PHASE_APP");
-    PERF_CHECK_ARG(phase == 0 || (d_feat && d_h1 && (phase == PERF_PHASE_GEO || d_h2)), "NULL save buffer");
-    PERF_CHECK_ARG(args->d_packed_table && args->d_geo_mlp_half && args->d_app_mlp_half, "NULL table / weights");
-    PERF_CHECK_ARG(((uintptr_t)d_feat | (uintptr_t)d_h1 | (uintptr_t)d_h2) % 16 == 0 && (uintptr_t)d_rgb_half4 % 8 == 0, "misaligned buffer");
-    RenderArgs a; memset(&a, 0, sizeof(a));
-    uint64_t n_entries = 0;
-    int rc = build_level_table(&args->grid, &a.lt, &n_entries); if (rc) return rc;
-    PERF_CHECK_SUP(args->grid.n_levels == 16, "fused field kernel needs n_levels == 16 (got %u)", args->grid.n_levels);
-    a.table = (const uint2*)args->d_packed_table;
-    PERF_CHECK_ARG((uintptr_t)args->d_packed_table % 16 == 0, "misaligned table");
-    const PackedLayout pl = packed_layout(a.lt, n_entries);
-    for (uint32_t l = 0; l < pl.n_cell_levels; ++l) a.cells[l] = reinterpret_cast<const uint4*>(a.table + pl.cell_start[l]);
-    a.geo_w = (const __half*)args->d_geo_mlp_half; a.app_w = (const __half*)args->d_app_mlp_half;
-    for (int i = 0; i < 3; ++i) { a.aabb_min[i] = args->aabb[i]; a.aabb_ext[i] = args->aabb[3 + i] - args->aabb[i]; }
-    set_div_mode(a);
-    a.rays_o = d_rays_o; a.rays_d = d_rays_d;
-    a.s_feat = (uint4*)d_feat; a.s_h1 = (uint4*)d_h1; a.s_h2 = (uint4*)d_h2;
-    if (N == 0) return PERF_OK;
-    PackedFieldArgs p = {d_ray_indices, d_t_starts, d_t_ends, N, d_n_dev, d_sigma, (__half*)d_rgb_half4, d_x01};
-    cudaStream_t st = (cudaStream_t)stream;
-    rc = prepare_weights(a, st); if (rc) return rc;
-    const uint64_t n_tiles = (N + TILE - 1) / TILE;
-    const unsigned grid = (unsigned)(n_tiles < (uint64_t)num_sms() * 4 ? n_tiles : (uint64_t)num_sms() * 4);
-    const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
-    // BYTES: RE_TOTAL for the eval kernels (phase 0), RS_TOTAL for the saving ones
-#define PERF_PACKED_LAUNCH(BYTES, ...) do { \
-        auto k = __VA_ARGS__; \
-        static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
-        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
-        k<<<grid, TILE, BYTES, st>>>(a, p); } while (0)
-    if (fast) {
-        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<4, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 1>);
-        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 2>);
-    } else {
-        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<-1, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 1>);
-        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 2>);
-    }
-#undef PERF_PACKED_LAUNCH
-    PERF_LAUNCH_CHECK();
-    return PERF_OK;
+    return fields_packed(args, d_rays_o, d_rays_d, d_ray_indices, d_t_starts, d_t_ends, N, d_n_dev, phase, d_sigma, d_rgb_half4, d_x01,
+                         d_feat, d_h1, d_h2, nullptr, stream);
 }
 
 int perf_render_pano(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows, void* stream)
@@ -1103,6 +1279,47 @@ int perf_render_pano(const perf_render_args* args, const float* h_pose, int H, i
     a.H = H; a.W = W; a.row0 = row0; a.R = (uint64_t)rows * W;
     return launch_render(args, a, true, (cudaStream_t)stream);
 }
+
+// ---- surface normals (perfb200.h: perf_render_pano_normals and the others)
+#define PERF_NORMALS_FLAGS_OK(args) PERF_CHECK_SUP(((args)->flags & (PERF_FLAG_SIMT_MLP | PERF_FLAG_SCAN_KERNEL | PERF_FLAG_L0_SMEM | \
+                                                                   PERF_FLAG_TRAINING)) == 0, "normals: eval render on the ray-marching wgmma kernel only")
+
+int perf_render_pano_normals(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && h_pose && d_normal, "NULL pointer");
+    PERF_NORMALS_FLAGS_OK(args);
+    PERF_CHECK_ARG(H > 0 && W > 0 && row0 >= 0 && rows >= 0 && row0 + rows <= H, "bad panorama window H=%d W=%d row0=%d rows=%d", H, W, row0, rows);
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) a.pose_r[3 * r + c] = h_pose[4 * r + c]; a.pose_t[r] = h_pose[4 * r + 3]; }
+    a.H = H; a.W = W; a.row0 = row0; a.R = (uint64_t)rows * W;
+    a.normal = d_normal;
+    return launch_render(args, a, true, (cudaStream_t)stream, 0, true);
+}
+
+int perf_render_rays_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && d_rays_o && d_rays_d && d_normal, "NULL pointer");
+    PERF_NORMALS_FLAGS_OK(args);
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    a.rays_o = d_rays_o; a.rays_d = d_rays_d; a.R = R;
+    if (args->image_width > 0) {
+        PERF_CHECK_ARG(R % args->image_width == 0, "image_width=%u does not divide the %llu rays", args->image_width, (unsigned long long)R);
+        a.W = (int)args->image_width;
+    }
+    a.normal = d_normal;
+    return launch_render(args, a, false, (cudaStream_t)stream, 0, true);
+}
+
+int perf_fields_packed_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, const int64_t* d_ray_indices,
+                               const float* d_t_starts, const float* d_t_ends, uint64_t N, const int64_t* d_n_dev, float* d_sigma,
+                               void* d_rgb_half4, float* d_x01, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && d_normal, "NULL pointer");
+    PERF_NORMALS_FLAGS_OK(args);
+    return fields_packed(args, d_rays_o, d_rays_d, d_ray_indices, d_t_starts, d_t_ends, N, d_n_dev, 0, d_sigma, d_rgb_half4, d_x01,
+                         nullptr, nullptr, nullptr, d_normal, stream);
+}
+#undef PERF_NORMALS_FLAGS_OK
 
 #pragma GCC visibility pop
 }  // extern "C"

@@ -512,22 +512,27 @@ def _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, n_samples, near
 
 def render_rays(packed_table, geo_mlp_half, app_mlp_half, rays_o, rays_d, n_samples: int, near=1e-2, far=1.0,
                 aabb=(-1., -1., -1., 1., 1., 1.), training=False, jitter=None, bg_noise=None,
-                grid: GridConfig = PERF_GRID, simt=False, kernel="march", image_width: int = 0):
+                grid: GridConfig = PERF_GRID, simt=False, kernel="march", image_width: int = 0, normals: bool = False):
     """Fused render of explicit rays [R,3] -> (rgb [R,3], distance [R,1], opacity [R,1]).
-    ``image_width`` > 0 declares the rays a row-major image of that width (pixel-patch tiling)."""
+    ``image_width`` > 0 declares the rays a row-major image of that width (pixel-patch tiling).
+    ``normals``: also the ray normal [R,3] = sum w n (``perf_render_rays_normals``; eval march kernel only)."""
     rays_o, rays_d = _chk(rays_o, torch.float32, "rays_o"), _chk(rays_d, torch.float32, "rays_d")
     R, dev = rays_o.shape[0], rays_o.device
     rgb = torch.empty(R, 3, dtype=torch.float32, device=dev)
     dist = torch.empty(R, 1, dtype=torch.float32, device=dev)
     op = torch.empty(R, 1, dtype=torch.float32, device=dev)
+    nrm = torch.empty(R, 3, dtype=torch.float32, device=dev) if normals else None
     if R == 0:
-        return rgb, dist, op
+        return (rgb, dist, op, nrm) if normals else (rgb, dist, op)
     jitter = None if jitter is None else _chk(jitter, torch.float32, "jitter")
     bg_noise = None if bg_noise is None else _chk(bg_noise, torch.float32, "bg_noise")
     a = _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, n_samples, near, far, training, simt,
                      jitter, bg_noise, rgb, dist, op, grid, kernel)
     a.image_width = int(image_width) if image_width and R % int(image_width) == 0 else 0
     with torch.cuda.device(dev):
+        if normals:
+            _call(_L().perf_render_rays_normals, C.byref(a), _p(rays_o), _p(rays_d), R, _p(nrm), _stream())
+            return rgb, dist, op, nrm
         _call(_L().perf_render_rays, C.byref(a), _p(rays_o), _p(rays_d), R, _stream())
     return rgb, dist, op
 
@@ -557,8 +562,10 @@ def render_packed(packed_table, geo_mlp_half, app_mlp_half, rays_o, rays_d, ray_
 
 
 def render_occ(packed_table, geo_mlp_half, app_mlp_half, rays_o, rays_d, offsets, ray_indices, t_starts, t_ends,
-               early_stop_eps: float = 1e-4, aabb=(-1., -1., -1., 1., 1., 1.), grid: GridConfig = PERF_GRID):
-    """Eval render of packed intervals: perf_fields_packed (no saves) + perf_composite_packed_fwd (eval background)."""
+               early_stop_eps: float = 1e-4, aabb=(-1., -1., -1., 1., 1., 1.), grid: GridConfig = PERF_GRID, normals: bool = False):
+    """Eval render of packed intervals: perf_fields_packed (no saves) + perf_composite_packed_fwd (eval background).
+    ``normals``: perf_fields_packed_normals instead, and the ray normal [R,3] = sum w n (perf_accumulate_along_rays over the
+    composite's weights) as a fourth output."""
     rays_o, rays_d = _chk(rays_o, torch.float32, "rays_o"), _chk(rays_d, torch.float32, "rays_d")
     offsets, ray_indices = _chk(offsets, torch.int64, "offsets"), _chk(ray_indices, torch.int64, "ray_indices")
     t_starts, t_ends = _chk(t_starts, torch.float32, "t_starts"), _chk(t_ends, torch.float32, "t_ends")
@@ -566,23 +573,31 @@ def render_occ(packed_table, geo_mlp_half, app_mlp_half, rays_o, rays_d, offsets
     f32 = lambda *sh: torch.empty(*sh, dtype=torch.float32, device=dev)
     rgb, dist, op = f32(R, 3), f32(R, 1), f32(R, 1)
     if R == 0:
-        return rgb, dist, op
+        return (rgb, dist, op, f32(R, 3)) if normals else (rgb, dist, op)
     sigma, c16, x01 = f32(N), torch.empty(N, 4, dtype=torch.float16, device=dev), f32(N, 3)
     w, T, dacc, dl = f32(N), f32(N), f32(R), f32(R)
     a = _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, 1, 0.0, 1.0, False, False, None, None, rgb, dist, op, grid)
     with torch.cuda.device(dev):
-        _call(_L().perf_fields_packed, C.byref(a), _p(rays_o), _p(rays_d), _p(ray_indices), _p(t_starts), _p(t_ends), N, None, 0,
-              _p(sigma), _p(c16), _p(x01), None, None, None, _stream(), launches=2)
+        if normals:
+            n_s = f32(N, 3)
+            _call(_L().perf_fields_packed_normals, C.byref(a), _p(rays_o), _p(rays_d), _p(ray_indices), _p(t_starts), _p(t_ends), N, None,
+                  _p(sigma), _p(c16), _p(x01), _p(n_s), _stream(), launches=2)
+        else:
+            _call(_L().perf_fields_packed, C.byref(a), _p(rays_o), _p(rays_d), _p(ray_indices), _p(t_starts), _p(t_ends), N, None, 0,
+                  _p(sigma), _p(c16), _p(x01), None, None, None, _stream(), launches=2)
         _call(_L().perf_composite_packed_fwd, _p(offsets), _p(t_starts), _p(t_ends), _p(sigma), _p(c16), R, float(early_stop_eps), 0, None,
               _p(w), _p(T), _p(rgb), _p(dist), _p(op), _p(dacc), _p(dl), _stream())
+    if normals:
+        return rgb, dist, op, accumulate_along_rays(w, n_s, ray_indices, R)
     return rgb, dist, op
 
 
 def render_pano(packed_table, geo_mlp_half, app_mlp_half, pose, H: int, W: int, n_samples: int, near=1e-2, far=1.0,
                 row0: int = 0, rows: Optional[int] = None, aabb=(-1., -1., -1., 1., 1., 1.),
-                grid: GridConfig = PERF_GRID, simt=False, out=None, kernel="march"):
+                grid: GridConfig = PERF_GRID, simt=False, out=None, kernel="march", normals: bool = False):
     """Fused render of rows [row0,row0+rows) of an HxW equirect panorama (ray-gen inside the kernel).
-    Returns (rgb [rows,W,3], distance [rows,W,1], opacity [rows,W,1])."""
+    Returns (rgb [rows,W,3], distance [rows,W,1], opacity [rows,W,1]), with ``normals`` also the ray normal
+    [rows,W,3] = sum w n (``perf_render_pano_normals``; ``out`` may then hold four tensors)."""
     rows = H - row0 if rows is None else rows
     dev = packed_table.device
     if out is None:
@@ -590,10 +605,14 @@ def render_pano(packed_table, geo_mlp_half, app_mlp_half, pose, H: int, W: int, 
         dist = torch.empty(rows, W, 1, dtype=torch.float32, device=dev)
         op = torch.empty(rows, W, 1, dtype=torch.float32, device=dev)
     else:
-        rgb, dist, op = out
+        rgb, dist, op = out[:3]
     a = _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, n_samples, near, far, False, simt,
                      None, None, rgb, dist, op, grid, kernel)
     with torch.cuda.device(dev):
+        if normals:
+            nrm = out[3] if out is not None and len(out) > 3 else torch.empty(rows, W, 3, dtype=torch.float32, device=dev)
+            _call(_L().perf_render_pano_normals, C.byref(a), _pose_array(pose), H, W, row0, rows, _p(nrm), _stream())
+            return rgb, dist, op, nrm
         _call(_L().perf_render_pano, C.byref(a), _pose_array(pose), H, W, row0, rows, _stream())
     return rgb, dist, op
 

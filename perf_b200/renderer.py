@@ -61,14 +61,23 @@ class FusedPanoRenderer:
 
     def render_rays(self, rays_o: torch.Tensor, rays_d: torch.Tensor, n_samples: int, near: Optional[float] = None,
                     far: Optional[float] = None, training: bool = False, jitter: Optional[torch.Tensor] = None,
-                    bg_noise: Optional[torch.Tensor] = None, simt: bool = False) -> dict:
+                    bg_noise: Optional[torch.Tensor] = None, simt: bool = False, normals: bool = False) -> dict:
+        """``normals``: also ``"normal"`` [R,3] = sum w n, the weighted density-gradient normal (include/perfb200.h
+        defines it; not normalised, its length is at most the opacity)."""
         self._ready()
         # [H, W, 3] ray images are tiled as pixel patches (same locality as render_pano)
         image_width = rays_o.shape[-2] if rays_o.dim() == 3 else 0
-        rgb, dist, op = ops.render_rays(self.packed, self.geo_half, self.app_half, rays_o.reshape(-1, 3), rays_d.reshape(-1, 3),
-                                        n_samples, self.near if near is None else near, self.far if far is None else far,
-                                        self.aabb, training, jitter, bg_noise, self.grid, simt, self.kernel, image_width)
-        return {"rgb": rgb, "distance": dist, "opacities": op, "is_valid": True}
+        out = ops.render_rays(self.packed, self.geo_half, self.app_half, rays_o.reshape(-1, 3), rays_d.reshape(-1, 3),
+                              n_samples, self.near if near is None else near, self.far if far is None else far,
+                              self.aabb, training, jitter, bg_noise, self.grid, simt, self.kernel, image_width, normals=normals)
+        return self._result(out)
+
+    @staticmethod
+    def _result(out) -> dict:
+        res = {"rgb": out[0], "distance": out[1], "opacities": out[2], "is_valid": True}
+        if len(out) > 3:
+            res["normal"] = out[3]
+        return res
 
     def render_packed(self, rays_o: torch.Tensor, rays_d: torch.Tensor, ray_indices: torch.Tensor, t_starts: torch.Tensor,
                       t_ends: torch.Tensor, simt: bool = False) -> dict:
@@ -80,30 +89,32 @@ class FusedPanoRenderer:
         return {"rgb": rgb, "distance": dist, "opacities": op, "is_valid": True}
 
     def render_occ(self, rays_o: torch.Tensor, rays_d: torch.Tensor, offsets: torch.Tensor, ray_indices: torch.Tensor,
-                   t_starts: torch.Tensor, t_ends: torch.Tensor, early_stop_eps: float = 1e-4) -> dict:
+                   t_starts: torch.Tensor, t_ends: torch.Tensor, early_stop_eps: float = 1e-4, normals: bool = False) -> dict:
         """Eval render of ALL intervals an occupancy sampler emitted (no visibility pre-pass): both fields at every
         interval in one launch (perf_fields_packed), then the per-ray composite with nerfacc's transmittance cut applied
         inside (perf_composite_packed_fwd) -- `nerf_renderer.py:145-197` without the second density evaluation."""
         self._ready()
-        rgb, dist, op = ops.render_occ(self.packed, self.geo_half, self.app_half, rays_o.reshape(-1, 3), rays_d.reshape(-1, 3),
-                                       offsets, ray_indices, t_starts, t_ends, early_stop_eps, self.aabb, self.grid)
-        return {"rgb": rgb, "distance": dist, "opacities": op, "is_valid": True}
+        out = ops.render_occ(self.packed, self.geo_half, self.app_half, rays_o.reshape(-1, 3), rays_d.reshape(-1, 3),
+                             offsets, ray_indices, t_starts, t_ends, early_stop_eps, self.aabb, self.grid, normals=normals)
+        return self._result(out)
 
     def render_pano(self, pose, H: int, W: int, n_samples: int, row0: int = 0, rows: Optional[int] = None,
-                    near: Optional[float] = None, far: Optional[float] = None, simt: bool = False, out=None) -> dict:
+                    near: Optional[float] = None, far: Optional[float] = None, simt: bool = False, out=None,
+                    normals: bool = False) -> dict:
         self._ready()
-        rgb, dist, op = ops.render_pano(self.packed, self.geo_half, self.app_half, pose, H, W, n_samples,
-                                        self.near if near is None else near, self.far if far is None else far,
-                                        row0, rows, self.aabb, self.grid, simt, out, self.kernel)
-        return {"rgb": rgb, "distance": dist, "opacities": op, "is_valid": True}
+        res = ops.render_pano(self.packed, self.geo_half, self.app_half, pose, H, W, n_samples,
+                              self.near if near is None else near, self.far if far is None else far,
+                              row0, rows, self.aabb, self.grid, simt, out, self.kernel, normals=normals)
+        return self._result(res)
 
     @torch.no_grad()
     def render(self, rays, query_keys=("rgb",), n_samples: int = 128) -> dict:
         """Drop-in for ``NeRFScene.render(rays, query_keys)``: ``rays`` has ``.o`` / ``.d`` of shape
-        [..., 3]; returns ``{key: tensor[..., C]}`` (eval-mode background rule)."""
+        [..., 3]; returns ``{key: tensor[..., C]}`` (eval-mode background rule).  ``"normal"`` is the weighted
+        surface normal [..., 3]."""
         pre_shape = list(rays.o.shape[:-1])
         o, d = rays.o.float(), rays.d.float()
         if o.dim() != 3:
             o, d = o.reshape(-1, 3), d.reshape(-1, 3)
-        out = self.render_rays(o, d, n_samples)
+        out = self.render_rays(o, d, n_samples, normals="normal" in query_keys)
         return {k: out[k].reshape(pre_shape + [-1]) for k in query_keys}

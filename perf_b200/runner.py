@@ -158,7 +158,10 @@ class CoreRunner:
     @torch.no_grad()
     def render_dense(self, n_poses=180, cam_type="pano", height=512, width=1024, write=True):
         """`core_exp_runner.py:223-246`.  With several ranks (torchrun) every frame is row-tiled over them and
-        gathered on rank 0.  Returns the uint8 colour frames on rank 0 (the reference's ``color_frames``)."""
+        gathered on rank 0.  Returns the uint8 colour frames on rank 0 (the reference's ``color_frames``).
+        Config key ``render_normals`` (default false): also write ``normal_{i}.png``, the weighted surface normal as
+        ``(n / |n| * 0.5 + 0.5) * 255`` (the reference's normal visualisation, `core_exp_runner.py:213`)."""
+        normals = bool(self.conf.get("render_normals", False))
         sampler = DenseTravelPoseSampler(self.pose_sampler, n_dense_poses=n_poses)
         out_dir = pjoin(self.exp_dir, "dense_images_new_" + cam_type)
         if self.is_main and write:
@@ -170,21 +173,27 @@ class CoreRunner:
             if cam_type == "pano":
                 pose[:3, :3] = torch.eye(3)
                 sl = parallel.shard_slice(height, rank, world)
-                out = self.scene.render_pano(pose, height, width, row0=sl.start, rows=sl.stop - sl.start)
+                out = (self.scene.render_pano(pose, height, width, row0=sl.start, rows=sl.stop - sl.start, normals=True) if normals
+                       else self.scene.render_pano(pose, height, width, row0=sl.start, rows=sl.stop - sl.start))
                 colors, distances = out["rgb"], out["distance"]
             else:
                 rays = gen_pers_rays(pose, fov=np.deg2rad(75.), res=height, device=self.device)
                 sl = parallel.shard_slice(height, rank, world)
-                out = self.scene.render(type(rays)(rays.o[sl], rays.d[sl]), query_keys=["rgb", "distance"])
+                out = self.scene.render(type(rays)(rays.o[sl], rays.d[sl]), query_keys=["rgb", "distance"] + (["normal"] if normals else []))
                 colors, distances = out["rgb"], out["distance"]
-            tile = parallel.gather_row_tiles(torch.cat([colors, distances], -1).contiguous(), height)
+            channels = [colors, distances] + ([out["normal"]] if normals else [])
+            tile = parallel.gather_row_tiles(torch.cat(channels, -1).contiguous(), height)
             if tile is None:
                 continue
-            colors, distances = tile[..., :3], tile[..., 3:]
+            colors, distances = tile[..., :3], tile[..., 3:4]
             frames.append((colors.clip(0., 1.) * 255.).cpu().numpy().astype(np.uint8))
             if write:
                 write_image(pjoin(out_dir, "image_{}.png".format(i)), colors * 255.)
                 write_image(pjoin(out_dir, "distance_{}.png".format(i)), colorize_single_channel_image(1. / distances))
+                if normals:
+                    n = tile[..., 4:7]
+                    n = n / n.norm(dim=-1, keepdim=True).clamp(min=1e-12)
+                    write_image(pjoin(out_dir, "normal_{}.png".format(i)), ((n * .5 + .5).clip(0., 1.) * 255.).byte())
         if self.is_main and write and frames:
             self._write_video(pjoin(out_dir, "video.mp4"), frames)
         return frames

@@ -426,8 +426,10 @@ class NeRFScene:
 
     @torch.no_grad()
     def render(self, rays: Rays, query_keys=("rgb",), sampling_requires_grad=False):
-        """`nerf.py:74-99`: eval-mode render of arbitrarily shaped rays -> {key: [..., C]}."""
+        """`nerf.py:74-99`: eval-mode render of arbitrarily shaped rays -> {key: [..., C]}.  ``"normal"`` in
+        ``query_keys`` adds the weighted density-gradient surface normal [..., 3] (both estimators)."""
         self._sync_fused()
+        normals = "normal" in query_keys
         rays_o, rays_d = rays.collapse()
         pre_shape = list(rays_o.shape[:-1])
         image = rays_o.dim() == 3                      # [H, W, 3] image of rays: keep the shape as a locality hint
@@ -439,20 +441,24 @@ class NeRFScene:
             est = self.estimator
             ri, ts, te = ops.occ_sample(est.binaries[0], est._aabb_list(), rays_o.contiguous(), rays_d.contiguous(), 0.0, 1.5,
                                         self.OCC_STEP, None)
-            out = self.fused.render_occ(rays_o, rays_d, ops.occ_sample.last_offsets, ri, ts, te, early_stop_eps=1e-4)
+            out = self.fused.render_occ(rays_o, rays_d, ops.occ_sample.last_offsets, ri, ts, te, early_stop_eps=1e-4, normals=normals)
         else:
-            out = self.fused.render_rays(rays_o_img if image else rays_o, rays_d_img if image else rays_d, self.estimator.n_samples)
+            out = self.fused.render_rays(rays_o_img if image else rays_o, rays_d_img if image else rays_d, self.estimator.n_samples,
+                                         normals=normals)
         return {k: out[k].reshape(pre_shape + [-1]) for k in query_keys}
 
     @torch.no_grad()
-    def render_pano(self, pose, height, width, row0=0, rows=None):
-        """render_dense inner loop (`core_exp_runner.py:229-238`) with ray generation fused in."""
+    def render_pano(self, pose, height, width, row0=0, rows=None, normals=False):
+        """render_dense inner loop (`core_exp_runner.py:229-238`) with ray generation fused in.  ``normals``: also
+        ``"normal"`` [rows, width, 3]."""
         self._sync_fused()
         if self.estimator_type == "occ":
             rows = height - row0 if rows is None else rows
             o, d = ops.raygen_pano(pose, height, width, row0, rows, device=self.device)
-            out = self.render(Rays(o, d), ["rgb", "distance", "opacities"])
+            out = self.render(Rays(o, d), ["rgb", "distance", "opacities"] + (["normal"] if normals else []))
             return {**out, "is_valid": True}
+        if normals:
+            return self.fused.render_pano(pose, height, width, self.estimator.n_samples, row0=row0, rows=rows, normals=True)
         return self.fused.render_pano(pose, height, width, self.estimator.n_samples, row0=row0, rows=rows)
 
     @torch.no_grad()
