@@ -139,27 +139,6 @@ __global__ void __launch_bounds__(256) pack_tables_kernel(const uint32_t* __rest
     }
 }
 
-// torch.linspace(start, end, steps)[i] in fp32 (ATen's symmetric formula), so that pixel centres
-// match utils/camera_utils.py:113-117 to the ulp.
-__device__ __forceinline__ float linspace_val(int i, int n)
-{
-    const float start = (float)(0.5 / (double)n), end = (float)(1.0 - 0.5 / (double)n);
-    if (n == 1) return start;
-    const float step = (end - start) / (float)(n - 1);
-    return (i < n / 2) ? __fadd_rn(start, __fmul_rn(step, (float)i)) : __fsub_rn(end, __fmul_rn(step, (float)(n - i - 1)));
-}
-
-// camera-space equirect direction of pixel (row, col): camera_utils.py:120-126,142-147
-__device__ __forceinline__ void pano_dir(int row, int col, int H, int W, float& dx, float& dy, float& dz)
-{
-    const float y = linspace_val(row, H), x = linspace_val(col, W);
-    const float beta = -(y - 0.5f) * 3.14159274101257324f;            // float32(np.pi)
-    const float alpha = -(x - 0.5f) * 6.28318548202514648f;           // float32(2 np.pi)
-    float sa, ca, sb, cb;
-    sincosf(alpha, &sa, &ca); sincosf(beta, &sb, &cb);
-    dx = ca * cb; dy = sa * cb; dz = sb;
-}
-
 struct Pose { float r[9]; float t[3]; };
 
 __global__ void raygen_pano_kernel(Pose pose, int H, int W, int row0, int rows, float* __restrict__ o, float* __restrict__ d)
@@ -168,31 +147,20 @@ __global__ void raygen_pano_kernel(Pose pose, int H, int W, int row0, int rows, 
     if (i >= (uint64_t)rows * W) return;
     int row = row0 + (int)(i / W), col = (int)(i % W);
     float cx, cy, cz; pano_dir(row, col, H, W, cx, cy, cz);
-    // apply_rot (camera_utils.py:44-46): d_world = R d
-    d[3 * i + 0] = pose.r[0] * cx + pose.r[1] * cy + pose.r[2] * cz;
-    d[3 * i + 1] = pose.r[3] * cx + pose.r[4] * cy + pose.r[5] * cz;
-    d[3 * i + 2] = pose.r[6] * cx + pose.r[7] * cy + pose.r[8] * cz;
+    rotate(pose.r, cx, cy, cz, d[3 * i + 0], d[3 * i + 1], d[3 * i + 2]);
     o[3 * i + 0] = pose.t[0]; o[3 * i + 1] = pose.t[1]; o[3 * i + 2] = pose.t[2];
 }
 
 // perspective camera rays, OpenCV convention: camera_utils.py:60-80 (cam_rays_cam_space) + :237-241
-__device__ __forceinline__ float linspace_sym(float start, float end, int i, int n)
-{
-    if (n == 1) return start;
-    const float step = (end - start) / (float)(n - 1);
-    return (i < n / 2) ? __fadd_rn(start, __fmul_rn(step, (float)i)) : __fsub_rn(end, __fmul_rn(step, (float)(n - i - 1)));
-}
 __global__ void raygen_pers_kernel(Pose pose, float span_x, float span_y, int H, int W, float* __restrict__ o, float* __restrict__ d)
 {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (uint64_t)H * W) return;
     const int row = (int)(i / W), col = (int)(i % W);
-    const float y = linspace_sym(-span_y, span_y, row, H), x = linspace_sym(-span_x, span_x, col, W);
+    const float y = linspace(-span_y, span_y, row, H), x = linspace(-span_x, span_x, col, W);
     const float n = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), 1.0f));
     const float cx = x / n, cy = y / n, cz = 1.0f / n;
-    d[3 * i + 0] = pose.r[0] * cx + pose.r[1] * cy + pose.r[2] * cz;
-    d[3 * i + 1] = pose.r[3] * cx + pose.r[4] * cy + pose.r[5] * cz;
-    d[3 * i + 2] = pose.r[6] * cx + pose.r[7] * cy + pose.r[8] * cz;
+    rotate(pose.r, cx, cy, cz, d[3 * i + 0], d[3 * i + 1], d[3 * i + 2]);
     o[3 * i + 0] = pose.t[0]; o[3 * i + 1] = pose.t[1]; o[3 * i + 2] = pose.t[2];
 }
 

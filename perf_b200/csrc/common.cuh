@@ -99,15 +99,24 @@ __host__ __device__ __forceinline__ uint32_t level_index(uint32_t gx, uint32_t g
 #define PERF_FDIV_RN(a, b) ((a) / (b))
 #endif
 
+// A level's cell frame at (x, y, z) (tcnn pos_fract): per axis pos = scale x + 0.5, g = its integer cell, p = fract(pos).
+// The interpolation weights and corner indices built on it stay with each caller.
+__host__ __device__ __forceinline__ void cell_frame(float scale, float x, float y, float z,
+                                                    uint32_t& gx, uint32_t& gy, uint32_t& gz, float& px, float& py, float& pz)
+{
+    const float sx = fmaf(scale, x, 0.5f), sy = fmaf(scale, y, 0.5f), sz = fmaf(scale, z, 0.5f);
+    const float fx = floorf(sx), fy = floorf(sy), fz = floorf(sz);
+    gx = (uint32_t)(int)fx; gy = (uint32_t)(int)fy; gz = (uint32_t)(int)fz;
+    px = sx - fx; py = sy - fy; pz = sz - fz;
+}
+
 __host__ __device__ __forceinline__ void level_corners(const LevelTable& lt, int l, float x, float y, float z, Corner8& c)
 {
     const float scale = lt.scale[l];
     const uint32_t res = lt.res[l], size = lt.size[l], off = lt.offset[l];
     const bool hashed = (lt.hashed_mask >> l) & 1u, pow2 = (lt.pow2_mask >> l) & 1u;
-    float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
-    float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
-    uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
-    float wx = px - fx, wy = py - fy, wz = pz - fz;
+    uint32_t gx, gy, gz; float wx, wy, wz;
+    cell_frame(scale, x, y, z, gx, gy, gz, wx, wy, wz);
     if (lt.smoothstep) {
         wx = wx * wx * (3.0f - 2.0f * wx); wy = wy * wy * (3.0f - 2.0f * wy); wz = wz * wz * (3.0f - 2.0f * wz);
     }
@@ -130,10 +139,8 @@ __host__ __device__ __forceinline__ void level_corners_fast(const LevelTable& lt
 {
     const float scale = lt.scale[l];
     const uint32_t res = lt.res[l], size = lt.size[l], off = lt.offset[l];
-    const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
-    const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
-    const uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
-    const float wx = px - fx, wy = py - fy, wz = pz - fz;
+    uint32_t gx, gy, gz; float wx, wy, wz;
+    cell_frame(scale, x, y, z, gx, gy, gz, wx, wy, wz);
     const float ox = 1.0f - wx, oy = 1.0f - wy, oz = 1.0f - wz;
     const float wxy[4] = {PERF_FMUL_RN(ox, oy), PERF_FMUL_RN(wx, oy), PERF_FMUL_RN(ox, wy), PERF_FMUL_RN(wx, wy)};
 #pragma unroll
@@ -187,10 +194,8 @@ __host__ __device__ __forceinline__ void level_corners_rel(const LevelTable& lt,
 {
     const float scale = lt.scale[l];
     const uint32_t res = lt.res[l], size = lt.size[l];
-    const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
-    const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
-    const uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
-    const float wx = px - fx, wy = py - fy, wz = pz - fz;
+    uint32_t gx, gy, gz; float wx, wy, wz;
+    cell_frame(scale, x, y, z, gx, gy, gz, wx, wy, wz);
     const float ox = 1.0f - wx, oy = 1.0f - wy, oz = 1.0f - wz;
     const float wxy[4] = {PERF_FMUL_RN(ox, oy), PERF_FMUL_RN(wx, oy), PERF_FMUL_RN(ox, wy), PERF_FMUL_RN(wx, wy)};
 #pragma unroll
@@ -221,10 +226,8 @@ __host__ __device__ __forceinline__ uint32_t level_cell_dense(const LevelTable& 
 {
     const float scale = lt.scale[l];
     const uint32_t res = lt.res[l];
-    const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
-    const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
-    const uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
-    const float wx = px - fx, wy = py - fy, wz = pz - fz;
+    uint32_t gx, gy, gz; float wx, wy, wz;
+    cell_frame(scale, x, y, z, gx, gy, gz, wx, wy, wz);
     const float ox = 1.0f - wx, oy = 1.0f - wy, oz = 1.0f - wz;
     const float wxy[4] = {PERF_FMUL_RN(ox, oy), PERF_FMUL_RN(wx, oy), PERF_FMUL_RN(ox, wy), PERF_FMUL_RN(wx, wy)};
 #pragma unroll
@@ -327,6 +330,54 @@ inline bool div_uniform_ok(float ext)
 {
     uint32_t bits; memcpy(&bits, &ext, 4);
     return (bits & 0x7FFFFFu) != 0x7FFFFFu && ext > 1e-30f && ext < 1e30f;
+}
+
+// ---------------------------------------------------------------- device: rays and sample positions (oracle/sampler.py)
+// The backward kernels do not save sample positions: they recompute them from the rays with these helpers and must reach
+// the forward's fp32 x01 bit for bit, or the gradients land in other cells.
+// Fixed-S sampling: sample k of a ray covers [fixed_s_t(k), fixed_s_t(k + 1)), t(k) = near + (k + jit) step with
+// step = (far - near) / S.
+__host__ __device__ __forceinline__ float fixed_s_step(float near, float far, uint32_t S) { return PERF_FDIV_RN(PERF_FSUB_RN(far, near), (float)S); }
+__host__ __device__ __forceinline__ float fixed_s_t(float near, float step, uint32_t k, float jit)
+{
+    return PERF_FADD_RN(near, PERF_FMUL_RN(PERF_FADD_RN((float)k, jit), step));
+}
+// One axis of the sample midpoint o + d (ts + te) / 2, with tsum = ts + te (ngp_nerf.py:137-140)
+__host__ __device__ __forceinline__ float sample_midpoint(float o, float d, float tsum) { return PERF_FADD_RN(o, PERF_FMUL_RN(d, tsum) * 0.5f); }
+// One axis of the box [lo, lo + ext] mapped to [0, 1].  The forward field kernels divide with div_uniform() instead (same
+// subtraction): both divisions round correctly, so they agree bit for bit whenever div_uniform_ok() holds for every extent
+// (otherwise div_uniform() takes this division itself), and the backward relies on that.
+__host__ __device__ __forceinline__ float to_unit(float p, float lo, float ext) { return PERF_FDIV_RN(PERF_FSUB_RN(p, lo), ext); }
+
+// torch.linspace(start, end, n)[i] in fp32 (ATen's symmetric formula), so that pixel centres match
+// utils/camera_utils.py:113-117 to the ulp.
+__host__ __device__ __forceinline__ float linspace(float start, float end, int i, int n)
+{
+    if (n == 1) return start;
+    const float step = (end - start) / (float)(n - 1);
+    return (i < n / 2) ? PERF_FADD_RN(start, PERF_FMUL_RN(step, (float)i)) : PERF_FSUB_RN(end, PERF_FMUL_RN(step, (float)(n - i - 1)));
+}
+// pixel-centre coordinate of pixel i of n in (0, 1)
+__host__ __device__ __forceinline__ float linspace_val(int i, int n)
+{
+    return linspace((float)(0.5 / (double)n), (float)(1.0 - 0.5 / (double)n), i, n);
+}
+// camera-space equirect direction of pixel (row, col): camera_utils.py:120-126,142-147
+__host__ __device__ __forceinline__ void pano_dir(int row, int col, int H, int W, float& dx, float& dy, float& dz)
+{
+    const float y = linspace_val(row, H), x = linspace_val(col, W);
+    const float beta = -(y - 0.5f) * 3.14159274101257324f;            // float32(np.pi)
+    const float alpha = -(x - 0.5f) * 6.28318548202514648f;           // float32(2 np.pi)
+    float sa, ca, sb, cb;
+    sincosf(alpha, &sa, &ca); sincosf(beta, &sb, &cb);
+    dx = ca * cb; dy = sa * cb; dz = sb;
+}
+// apply_rot (camera_utils.py:44-46): d_world = R c, R row-major 3x3
+__host__ __device__ __forceinline__ void rotate(const float (&r)[9], float cx, float cy, float cz, float& dx, float& dy, float& dz)
+{
+    dx = r[0] * cx + r[1] * cy + r[2] * cz;
+    dy = r[3] * cx + r[4] * cy + r[5] * cz;
+    dz = r[6] * cx + r[7] * cy + r[8] * cz;
 }
 
 // ---------------------------------------------------------------- device: wgmma / mbarrier PTX

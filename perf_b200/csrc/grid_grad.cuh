@@ -28,6 +28,7 @@ __host__ __device__ __forceinline__ void level_frame(const LevelTable& lt, int l
     uint32_t g[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
+        // common.cuh::cell_frame per axis, kept inline: calling it changes the register allocation of encoding_grad.cu
         const float pos = fmaf(scale, in[d], 0.5f), fl = floorf(pos), p = pos - fl;
         g[d] = (uint32_t)(int)fl;
         if (lt.smoothstep) { f.s[d] = p * p * (3.0f - 2.0f * p); f.ds[d] = 6.0f * p * (1.0f - p); f.dds[d] = 6.0f - 12.0f * p; }

@@ -246,14 +246,13 @@ __host__ __device__ __forceinline__ void bwd_phase_dfeat(const MlpBwdArgs& a, ui
 __device__ __forceinline__ void scatter_fine_levels(const ScatterCtx& c, uint64_t row, const float (&v)[32])
 {
     const uint64_t ray = row % c.R; const uint32_t k = (uint32_t)(row / c.R);
-    const float step = __fdiv_rn(__fsub_rn(c.far, c.near), (float)c.S);
+    const float step = fixed_s_step(c.near, c.far, c.S);
     const float jit = c.jitter ? c.jitter[ray] : 0.f;
-    const float ts = __fadd_rn(c.near, __fmul_rn(__fadd_rn((float)k, jit), step));
-    const float te = __fadd_rn(c.near, __fmul_rn(__fadd_rn((float)(k + 1), jit), step));
+    const float ts = fixed_s_t(c.near, step, k, jit), te = fixed_s_t(c.near, step, k + 1, jit);
     const float tsum = __fadd_rn(ts, te);
-    const float x = __fdiv_rn(__fsub_rn(__fadd_rn(c.rays_o[3 * ray], __fmul_rn(c.rays_d[3 * ray], tsum) * 0.5f), c.aabb_min[0]), c.aabb_ext[0]);
-    const float y = __fdiv_rn(__fsub_rn(__fadd_rn(c.rays_o[3 * ray + 1], __fmul_rn(c.rays_d[3 * ray + 1], tsum) * 0.5f), c.aabb_min[1]), c.aabb_ext[1]);
-    const float z = __fdiv_rn(__fsub_rn(__fadd_rn(c.rays_o[3 * ray + 2], __fmul_rn(c.rays_d[3 * ray + 2], tsum) * 0.5f), c.aabb_min[2]), c.aabb_ext[2]);
+    const float x = to_unit(sample_midpoint(c.rays_o[3 * ray], c.rays_d[3 * ray], tsum), c.aabb_min[0], c.aabb_ext[0]);
+    const float y = to_unit(sample_midpoint(c.rays_o[3 * ray + 1], c.rays_d[3 * ray + 1], tsum), c.aabb_min[1], c.aabb_ext[1]);
+    const float z = to_unit(sample_midpoint(c.rays_o[3 * ray + 2], c.rays_d[3 * ray + 2], tsum), c.aabb_min[2], c.aabb_ext[2]);
 #pragma unroll
     for (int l = 8; l < 16; ++l) {                             // register indices of v must be compile-time: n_coarse == 8, 16 levels
         const float gx = v[2 * l], gy = v[2 * l + 1];

@@ -68,7 +68,7 @@ __host__ __device__ __forceinline__ void occ_march_ray(const OccArgs& a, uint64_
             for (int j = 0; j < 32 * PERF_OCC_MASK_WORDS; ++j) {
                 if ((a.masks[slot * PERF_OCC_MASK_WORDS + (j >> 5)] >> (j & 31)) & 1u) {
                     const uint32_t kk = k_first + (uint32_t)j;
-                    const float ts = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)kk, u), a.step));
+                    const float ts = fixed_s_t(a.near, a.step, kk, u);
                     if (a.capacity == 0 || pos < a.capacity) { a.ray_indices[pos] = (int64_t)ray; a.t_starts[pos] = ts; a.t_ends[pos] = PERF_FADD_RN(ts, a.step); }
                     ++pos;
                 }
@@ -76,7 +76,7 @@ __host__ __device__ __forceinline__ void occ_march_ray(const OccArgs& a, uint64_
             k = k_end;                                         // skip the march below
         }
         for (; k < k_end; ++k) {
-            const float ts = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)k, u), a.step));
+            const float ts = fixed_s_t(a.near, a.step, k, u);
             const float mid = PERF_FADD_RN(ts, half_step);
             if (mid > tf) break;
             if (mid < tn) continue;
@@ -86,7 +86,7 @@ __host__ __device__ __forceinline__ void occ_march_ray(const OccArgs& a, uint64_
                 const float p = PERF_FADD_RN(o[i], PERF_FMUL_RN(d[i], mid));
                 pnt[i] = p;
                 const int res = i == 0 ? a.rx : (i == 1 ? a.ry : a.rz);
-                int ci = (int)floorf(PERF_FMUL_RN(PERF_FDIV_RN(PERF_FSUB_RN(p, a.amin[i]), a.aext[i]), (float)res));
+                int ci = (int)floorf(PERF_FMUL_RN(to_unit(p, a.amin[i], a.aext[i]), (float)res));
                 c[i] = ci < 0 ? 0 : (ci > res - 1 ? res - 1 : ci);
             }
             if (a.binaries[((int64_t)c[0] * a.ry + c[1]) * a.rz + c[2]]) {

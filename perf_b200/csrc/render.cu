@@ -181,14 +181,6 @@ __device__ __forceinline__ void out_dots_const(const uint32_t (&p)[16], float2 (
     }
 }
 
-__device__ __forceinline__ float linspace_val_r(int i, int n)
-{
-    const float start = (float)(0.5 / (double)n), end = (float)(1.0 - 0.5 / (double)n);
-    if (n == 1) return start;
-    const float step = (end - start) / (float)(n - 1);
-    return (i < n / 2) ? __fadd_rn(start, __fmul_rn(step, (float)i)) : __fsub_rn(end, __fmul_rn(step, (float)(n - i - 1)));
-}
-
 // Inclusive scan of NV values along the ray across the whole CTA tile (and across the tiles of
 // a unit through `carry`).  Lanes are consecutive samples; a ray may start anywhere.
 //   k        : index of this sample inside its ray
@@ -261,6 +253,17 @@ __device__ __forceinline__ void ray_scan(float (&val)[NV], float (&excl)[NV], ui
 #endif
 constexpr int PATCH_W = PATCH_WW * PATCH_WX, PATCH_H = PATCH_WH * PATCH_WY;
 static_assert(PATCH_WW * PATCH_WH == 32 && PATCH_WX * PATCH_WY == 4, "a warp is 32 pixels, a tile 4 warps");
+
+// Tiles of an image-shaped launch: patch_cols(W) across an image W pixels wide, patch_rows(rows) down one `rows` high.
+__host__ __device__ __forceinline__ int patch_cols(int W) { return (W + PATCH_W - 1) / PATCH_W; }
+__host__ __device__ __forceinline__ int patch_rows(int rows) { return (rows + PATCH_H - 1) / PATCH_H; }
+// Pixel (prow, pcol) of lane `lane` of warp `warp` in patch tile `tile`, tiles_x = patch_cols(W) tiles per image row.
+__device__ __forceinline__ void patch_pixel(uint64_t tile, uint32_t tiles_x, int warp, int lane, int& prow, int& pcol)
+{
+    const int ty = (int)(tile / tiles_x), tx = (int)(tile % tiles_x);
+    prow = ty * PATCH_H + (warp / PATCH_WX) * PATCH_WH + lane / PATCH_WW;
+    pcol = tx * PATCH_W + (warp % PATCH_WX) * PATCH_WW + lane % PATCH_WW;
+}
 
 struct RenderSmem {
     uint8_t *sA, *sAg, *sAa, *sH, *sW1g, *sW1a, *sW2a;
@@ -504,6 +507,7 @@ __device__ __forceinline__ void normal_level(const RenderArgs& a, int l, float x
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] = unpack_half2(__ldg(&a.table[f.idx[k]].x));
     } else {
+        // cell_frame's fract, kept inline: calling it changes the NORMAL kernels' SASS
         const float scale = a.lt.scale[l];
         const float in[3] = {x, y, z};
 #pragma unroll
@@ -671,7 +675,7 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
     stage_weights_bulk<false>(smem, tid);            // W1 density | W1 colour | W2 colour operand images, one bulk copy
 
     const uint32_t S = a.S;
-    const float step = __fdiv_rn(__fsub_rn(a.far, a.near), (float)S);
+    const float step = fixed_s_step(a.near, a.far, S);
     const uint64_t n_units = (a.R + a.rays_per_unit - 1) / a.rays_per_unit;
     uint32_t tile_counter = 0;
 
@@ -689,7 +693,8 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
             if (valid) {
                 if constexpr (PANO) {
                     const int row = a.row0 + (int)(ray / (uint64_t)a.W), col = (int)(ray % (uint64_t)a.W);
-                    const float yy = linspace_val_r(row, a.H), xx = linspace_val_r(col, a.W);
+                    const float yy = linspace_val(row, a.H), xx = linspace_val(col, a.W);
+                    // pano_dir + rotate (common.cuh), kept inline here and below: calling them changes the render kernels' SASS
                     const float beta = -(yy - 0.5f) * 3.14159274101257324f;
                     const float alpha = -(xx - 0.5f) * 6.28318548202514648f;
                     float sa, ca, sb, cb;
@@ -705,16 +710,12 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
                 }
                 if (a.training && a.jitter) jit = a.jitter[ray];
             }
-            const float ts = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)k, jit), step));
-            const float te = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)(k + 1), jit), step));
+            const float ts = fixed_s_t(a.near, step, k, jit), te = fixed_s_t(a.near, step, k + 1, jit);
             const float tsum = __fadd_rn(ts, te);
-            const float px = __fadd_rn(ox, __fmul_rn(dx, tsum) * 0.5f);
-            const float py = __fadd_rn(oy, __fmul_rn(dy, tsum) * 0.5f);
-            const float pz = __fadd_rn(oz, __fmul_rn(dz, tsum) * 0.5f);
-            // ngp_nerf.py:137-140
-            const float x = __fdiv_rn(__fsub_rn(px, a.aabb_min[0]), a.aabb_ext[0]);
-            const float y = __fdiv_rn(__fsub_rn(py, a.aabb_min[1]), a.aabb_ext[1]);
-            const float z = __fdiv_rn(__fsub_rn(pz, a.aabb_min[2]), a.aabb_ext[2]);
+            const float px = sample_midpoint(ox, dx, tsum), py = sample_midpoint(oy, dy, tsum), pz = sample_midpoint(oz, dz, tsum);
+            const float x = to_unit(px, a.aabb_min[0], a.aabb_ext[0]);
+            const float y = to_unit(py, a.aabb_min[1], a.aabb_ext[1]);
+            const float z = to_unit(pz, a.aabb_min[2], a.aabb_ext[2]);
             const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
 
             float sigma, cr, cg, cb;
@@ -792,17 +793,18 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
     }
 
     const uint32_t S = a.S;
+    // fixed_s_step, kept inline: calling it changes this kernel's SASS
     const float step = __fdiv_rn(__fsub_rn(a.far, a.near), (float)S);
     const float rext0 = __frcp_rn(a.aabb_ext[0]), rext1 = __frcp_rn(a.aabb_ext[1]), rext2 = __frcp_rn(a.aabb_ext[2]);
     // PANO, or explicit rays that form a row-major image of width a.W (perf_render_args.image_width):
     // tiles are 16x8 pixel patches; otherwise 128 consecutive rays
     const bool patch = PANO || a.W > 0;
     const int rows = patch ? (int)(a.R / (uint64_t)a.W) : 0;
-    const uint32_t tiles_x = patch ? (uint32_t)((a.W + PATCH_W - 1) / PATCH_W) : 0u;
+    const uint32_t tiles_x = patch ? (uint32_t)patch_cols(a.W) : 0u;
     const uint32_t seg = (PANO || patch || a.pk_offsets != nullptr || a.seg == 0) ? 1u : a.seg;
     const uint32_t rpt = TILE / seg, kps = S / seg;                 // rays per tile, samples per segment
     const uint32_t my_seg = (uint32_t)tid / rpt;
-    const uint64_t n_tiles = patch ? (uint64_t)tiles_x * (uint64_t)((rows + PATCH_H - 1) / PATCH_H) : (a.R + rpt - 1) / rpt;
+    const uint64_t n_tiles = patch ? (uint64_t)tiles_x * (uint64_t)patch_rows(rows) : (a.R + rpt - 1) / rpt;
 
     for (uint64_t work = blockIdx.x; work < n_tiles; work += gridDim.x) {
         // Image-shaped work is dealt out in a scattered order: the tiles in flight at any moment (4 per SM) are spread over
@@ -813,13 +815,12 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
         uint64_t ray; bool valid;
         float ox = 0.f, oy = 0.f, oz = 0.f, dx = 1.f, dy = 0.f, dz = 0.f, jit = 0.f;
         if constexpr (PANO) {
-            const int ty = (int)(tile / tiles_x), tx = (int)(tile % tiles_x);
-            const int prow = ty * PATCH_H + (warp / PATCH_WX) * PATCH_WH + lane / PATCH_WW;   // row inside the window
-            const int pcol = tx * PATCH_W + (warp % PATCH_WX) * PATCH_WW + lane % PATCH_WW;
+            int prow, pcol;                                                               // prow: row inside the window
+            patch_pixel(tile, tiles_x, warp, lane, prow, pcol);
             valid = prow < rows && pcol < a.W;
             ray = (uint64_t)prow * (uint64_t)a.W + (uint64_t)pcol;
             if (valid) {
-                const float yy = linspace_val_r(a.row0 + prow, a.H), xx = linspace_val_r(pcol, a.W);
+                const float yy = linspace_val(a.row0 + prow, a.H), xx = linspace_val(pcol, a.W);
                 const float beta = -(yy - 0.5f) * 3.14159274101257324f;
                 const float alpha = -(xx - 0.5f) * 6.28318548202514648f;
                 float sa, ca, sb, cb;
@@ -832,9 +833,8 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             }
         } else {
             if (patch) {
-                const int ty = (int)(tile / tiles_x), tx = (int)(tile % tiles_x);
-                const int prow = ty * PATCH_H + (warp / PATCH_WX) * PATCH_WH + lane / PATCH_WW;
-                const int pcol = tx * PATCH_W + (warp % PATCH_WX) * PATCH_WW + lane % PATCH_WW;
+                int prow, pcol;
+                patch_pixel(tile, tiles_x, warp, lane, prow, pcol);
                 valid = prow < rows && pcol < a.W;
                 ray = (uint64_t)prow * (uint64_t)a.W + (uint64_t)pcol;
             } else {
@@ -875,13 +875,10 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             if (!PANO && a.pk_offsets != nullptr) {
                 ts = live ? a.pk_ts[pk_base + k] : 0.f; te = live ? a.pk_te[pk_base + k] : 0.f;
             } else {
-                ts = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)k, jit), step));
-                te = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)(k + 1), jit), step));
+                ts = fixed_s_t(a.near, step, k, jit); te = fixed_s_t(a.near, step, k + 1, jit);
             }
             const float tsum = __fadd_rn(ts, te);
-            const float px = __fadd_rn(ox, __fmul_rn(dx, tsum) * 0.5f);
-            const float py = __fadd_rn(oy, __fmul_rn(dy, tsum) * 0.5f);
-            const float pz = __fadd_rn(oz, __fmul_rn(dz, tsum) * 0.5f);
+            const float px = sample_midpoint(ox, dx, tsum), py = sample_midpoint(oy, dy, tsum), pz = sample_midpoint(oz, dz, tsum);
             const float x = div_uniform(__fsub_rn(px, a.aabb_min[0]), a.aabb_ext[0], rext0, a.div_generic != 0u);
             const float y = div_uniform(__fsub_rn(py, a.aabb_min[1]), a.aabb_ext[1], rext1, a.div_generic != 0u);
             const float z = div_uniform(__fsub_rn(pz, a.aabb_min[2]), a.aabb_ext[2], rext2, a.div_generic != 0u);
@@ -951,6 +948,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             const float one_m = 1.f - acc_w;
             float dist = acc_d, r = acc_r, g = acc_g, b = acc_b;
             if constexpr (SAVE != 0) { a.s_dacc[ray] = acc_d; a.s_dl[ray] = dl_uni * (1.f / 3.f) + 2.f * dl_bi; }
+            // the same background as render_kernel's; a shared helper changes this kernel's SASS
             if (a.training) {                                     // nerf_renderer.py:192-194
                 float n0 = 0.f, n1 = 0.f, n2 = 0.f, n3 = 0.f;
                 if (a.bg_noise) { n0 = a.bg_noise[4 * ray]; n1 = a.bg_noise[4 * ray + 1]; n2 = a.bg_noise[4 * ray + 2]; n3 = a.bg_noise[4 * ray + 3]; }
@@ -1009,9 +1007,9 @@ __global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_con
         if (valid) {
             const int64_t ray = p.ray_indices[n];
             const float tsum = __fadd_rn(p.ts[n], p.te[n]);
-            const float px = __fadd_rn(a.rays_o[3 * ray], __fmul_rn(a.rays_d[3 * ray], tsum) * 0.5f);
-            const float py = __fadd_rn(a.rays_o[3 * ray + 1], __fmul_rn(a.rays_d[3 * ray + 1], tsum) * 0.5f);
-            const float pz = __fadd_rn(a.rays_o[3 * ray + 2], __fmul_rn(a.rays_d[3 * ray + 2], tsum) * 0.5f);
+            const float px = sample_midpoint(a.rays_o[3 * ray], a.rays_d[3 * ray], tsum);
+            const float py = sample_midpoint(a.rays_o[3 * ray + 1], a.rays_d[3 * ray + 1], tsum);
+            const float pz = sample_midpoint(a.rays_o[3 * ray + 2], a.rays_d[3 * ray + 2], tsum);
             x = div_uniform(__fsub_rn(px, a.aabb_min[0]), a.aabb_ext[0], rext0, a.div_generic != 0u);
             y = div_uniform(__fsub_rn(py, a.aabb_min[1]), a.aabb_ext[1], rext1, a.div_generic != 0u);
             z = div_uniform(__fsub_rn(pz, a.aabb_min[2]), a.aabb_ext[2], rext2, a.div_generic != 0u);
@@ -1040,13 +1038,6 @@ static int prepare_weights(const RenderArgs& a, cudaStream_t stream)
     return PERF_OK;
 }
 
-// div_uniform()'s precondition: no box extent with an all-ones significand (Markstein's exception) or out of the normal range
-static void set_div_mode(RenderArgs& a)
-{
-    a.div_generic = 0u;
-    for (int i = 0; i < 3; ++i) if (!div_uniform_ok(a.aabb_ext[i])) a.div_generic = 1u;
-}
-
 static uint32_t gcd_u32(uint32_t a, uint32_t b) { while (b) { uint32_t t = a % b; a = b; b = t; } return a; }
 
 // Dynamic shared memory of a field kernel and its shared-memory carveout: the smallest that holds `ctas` resident CTAs (the
@@ -1068,24 +1059,49 @@ static int set_smem(K k, int bytes, int ctas)
     return PERF_OK;
 }
 
-// normals: a.normal is set (it shares its slot with a.s_toff, so only this flag selects the NORMAL kernels)
-static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano, cudaStream_t stream, int save = 0, bool normals = false)
+// Launch of field kernel K with `bytes` of dynamic shared memory; set_smem (4 CTAs / SM) runs once per device and kernel.
+template <auto K, class... P>
+static int launch_field(int bytes, unsigned grid, cudaStream_t stream, const P&... p)
+{
+    static thread_local int attr_dev = -1;
+    int dev = 0; PERF_CUDA(cudaGetDevice(&dev));
+    if (attr_dev != dev) { const int rc = set_smem(K, bytes, 4); if (rc) return rc; attr_dev = dev; }
+    K<<<grid, TILE, bytes, stream>>>(p...);
+    return PERF_OK;
+}
+
+// The part of RenderArgs every field kernel needs: level table, packed table and its cell-major copies, weights, aabb and
+// div_uniform()'s mode.  fast: PeRF's grid (4 dense + 12 hashed levels, all dense levels copied cell-major) and the caller
+// did not ask for generic addressing.
+static int init_field_args(const perf_render_args* args, RenderArgs& a, bool& fast)
 {
     PERF_CHECK_ARG(args->d_packed_table && args->d_geo_mlp_half && args->d_app_mlp_half, "NULL table / weights");
-    PERF_CHECK_ARG(args->d_rgb && args->d_distance, "NULL output");
-    PERF_CHECK_ARG(args->n_samples >= 1 && args->n_samples <= 4096, "n_samples=%u not in [1,4096]", args->n_samples);
-    PERF_CHECK_ARG(args->far > args->near, "far <= near");
-    PERF_CHECK_ARG((uintptr_t)args->d_packed_table % 16 == 0 && (uintptr_t)args->d_geo_mlp_half % 16 == 0 && (uintptr_t)args->d_app_mlp_half % 16 == 0, "misaligned table / weights");
+    PERF_CHECK_ARG((uintptr_t)args->d_packed_table % 16 == 0, "misaligned table");
     uint64_t n_entries = 0;
-    int rc = build_level_table(&args->grid, &a.lt, &n_entries); if (rc) return rc;
-    PERF_CHECK_SUP(args->grid.n_levels == 16, "fused renderer needs n_levels == 16 (got %u)", args->grid.n_levels);
+    const int rc = build_level_table(&args->grid, &a.lt, &n_entries); if (rc) return rc;
+    PERF_CHECK_SUP(args->grid.n_levels == 16, "fused field kernels need n_levels == 16 (got %u)", args->grid.n_levels);
     a.table = (const uint2*)args->d_packed_table;
     const PackedLayout pl = packed_layout(a.lt, n_entries);
     for (uint32_t l = 0; l < pl.n_cell_levels; ++l) a.cells[l] = reinterpret_cast<const uint4*>(a.table + pl.cell_start[l]);
     a.geo_w = (const __half*)args->d_geo_mlp_half; a.app_w = (const __half*)args->d_app_mlp_half;
     for (int i = 0; i < 3; ++i) { a.aabb_min[i] = args->aabb[i]; a.aabb_ext[i] = args->aabb[3 + i] - args->aabb[i]; }
+    // div_uniform()'s precondition: no box extent with an all-ones significand (Markstein's exception) or out of the normal range
+    a.div_generic = 0u;
+    for (int i = 0; i < 3; ++i) if (!div_uniform_ok(a.aabb_ext[i])) a.div_generic = 1u;
+    fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
+    return PERF_OK;
+}
+
+// normals: a.normal is set (it shares its slot with a.s_toff, so only this flag selects the NORMAL kernels)
+static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano, cudaStream_t stream, int save = 0, bool normals = false)
+{
+    PERF_CHECK_ARG(args->d_rgb && args->d_distance, "NULL output");
+    PERF_CHECK_ARG(args->n_samples >= 1 && args->n_samples <= 4096, "n_samples=%u not in [1,4096]", args->n_samples);
+    PERF_CHECK_ARG(args->far > args->near, "far <= near");
+    PERF_CHECK_ARG((uintptr_t)args->d_geo_mlp_half % 16 == 0 && (uintptr_t)args->d_app_mlp_half % 16 == 0, "misaligned weights");
+    bool fast = false;
+    int rc = init_field_args(args, a, fast); if (rc) return rc;
     a.S = args->n_samples; a.near = args->near; a.far = args->far;
-    set_div_mode(a);
     a.training = (args->flags & PERF_FLAG_TRAINING) ? 1u : 0u;
     a.jitter = args->d_jitter; a.bg_noise = args->d_bg_noise;
     a.rgb = args->d_rgb; a.distance = args->d_distance; a.opacity = args->d_opacity;
@@ -1099,7 +1115,7 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
 #define PERF_TILE_SCATTER 1
 #endif
     if (scan) n_work = (a.R + a.rays_per_unit - 1) / a.rays_per_unit;
-    else if (pano || a.W > 0) n_work = (uint64_t)((a.W + PATCH_W - 1) / PATCH_W) * (uint64_t)(((int)(a.R / (uint64_t)a.W) + PATCH_H - 1) / PATCH_H);
+    else if (pano || a.W > 0) n_work = (uint64_t)patch_cols(a.W) * (uint64_t)patch_rows((int)(a.R / (uint64_t)a.W));
     else {
         const uint32_t rpt = TILE / (a.seg ? a.seg : 1u);
         n_work = (a.R + rpt - 1) / rpt;
@@ -1113,25 +1129,19 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         a.tile_mul = m % (uint32_t)n_work;
     }
     rc = prepare_weights(a, stream); if (rc) return rc;     // constant-bank output weights + operand images (c_wout, g_wimg)
-    // BYTES: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RE_LAUNCH_N for their normals twins, RS_LAUNCH for the others
-#define PERF_RENDER_LAUNCH(BYTES, ...) do { \
-        auto k = __VA_ARGS__; \
-        static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
-        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
-        k<<<grid, TILE, BYTES, stream>>>(a); } while (0)
-    const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;   // PeRF's grid: 4 dense + 12 hashed levels
+    // bytes: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RE_LAUNCH_N for their normals twins, RS_LAUNCH for the others
     if (normals) {                                                // surface normals: eval march kernel only (the callers refuse the rest)
-        if (fast) { if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<true, false, 4, 0, false, true>); else PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<false, false, 4, 0, false, true>); }
-        else      { if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<true, false, -1, 0, false, true>); else PERF_RENDER_LAUNCH(RE_LAUNCH_N, render_march_kernel<false, false, -1, 0, false, true>); }
+        if (fast) rc = pano ? launch_field<render_march_kernel<true, false, 4, 0, false, true>>(RE_LAUNCH_N, grid, stream, a) : launch_field<render_march_kernel<false, false, 4, 0, false, true>>(RE_LAUNCH_N, grid, stream, a);
+        else      rc = pano ? launch_field<render_march_kernel<true, false, -1, 0, false, true>>(RE_LAUNCH_N, grid, stream, a) : launch_field<render_march_kernel<false, false, -1, 0, false, true>>(RE_LAUNCH_N, grid, stream, a);
     } else if (save != 0) {
         PERF_CHECK_SUP(!pano && !simt && !scan, "training forward runs on the ray-marching tensor-core kernel only");
-        if (fast) { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, 4, 2>); }
-        else      { if (save == 1) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, false, -1, 2>); }
+        if (fast) rc = save == 1 ? launch_field<render_march_kernel<false, false, 4, 1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, 4, 2>>(RS_LAUNCH, grid, stream, a);
+        else      rc = save == 1 ? launch_field<render_march_kernel<false, false, -1, 1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, -1, 2>>(RS_LAUNCH, grid, stream, a);
     } else if (scan) {
-        if (pano) { if (simt) PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<true, true>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<true, false>); }
-        else      { if (simt) PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<false, true>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_kernel<false, false>); }
+        if (pano) rc = simt ? launch_field<render_kernel<true, true>>(RS_LAUNCH, grid, stream, a) : launch_field<render_kernel<true, false>>(RS_LAUNCH, grid, stream, a);
+        else      rc = simt ? launch_field<render_kernel<false, true>>(RS_LAUNCH, grid, stream, a) : launch_field<render_kernel<false, false>>(RS_LAUNCH, grid, stream, a);
     } else if (simt) {
-        if (pano) PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<true, true, -1>); else PERF_RENDER_LAUNCH(RS_LAUNCH, render_march_kernel<false, true, -1>);
+        rc = pano ? launch_field<render_march_kernel<true, true, -1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, true, -1>>(RS_LAUNCH, grid, stream, a);
     } else if (fast && pano && (args->flags & PERF_FLAG_L0_SMEM)) {
         auto k = render_march_kernel<true, false, 4, 0, true>;           // experiment: level 0 in shared memory (2 CTAs/SM)
         static thread_local int attr_dev0 = -1, per_sm0 = 1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_));
@@ -1144,11 +1154,11 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         const uint64_t slots0 = (uint64_t)num_sms() * (uint64_t)per_sm0;
         k<<<(unsigned)(n_work < slots0 ? n_work : slots0), TILE, RE_TOTAL_L0, stream>>>(a);
     } else if (fast) {
-        if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<true, false, 4>); else PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<false, false, 4>);
+        rc = pano ? launch_field<render_march_kernel<true, false, 4>>(RE_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, 4>>(RE_LAUNCH, grid, stream, a);
     } else {
-        if (pano) PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<true, false, -1>); else PERF_RENDER_LAUNCH(RE_LAUNCH, render_march_kernel<false, false, -1>);
+        rc = pano ? launch_field<render_march_kernel<true, false, -1>>(RE_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, -1>>(RE_LAUNCH, grid, stream, a);
     }
-#undef PERF_RENDER_LAUNCH
+    if (rc) return rc;
     PERF_LAUNCH_CHECK();
     return PERF_OK;
 }
@@ -1161,19 +1171,10 @@ static int fields_packed(const perf_render_args* args, const float* d_rays_o, co
     PERF_CHECK_ARG(args && d_rays_o && d_rays_d && d_ray_indices && d_t_starts && d_t_ends && d_sigma && d_rgb_half4 && d_x01, "NULL pointer");
     PERF_CHECK_ARG(phase == 0 || phase == PERF_PHASE_GEO || phase == PERF_PHASE_APP, "phase must be 0, PERF_PHASE_GEO or PERF_PHASE_APP");
     PERF_CHECK_ARG(phase == 0 || (d_feat && d_h1 && (phase == PERF_PHASE_GEO || d_h2)), "NULL save buffer");
-    PERF_CHECK_ARG(args->d_packed_table && args->d_geo_mlp_half && args->d_app_mlp_half, "NULL table / weights");
     PERF_CHECK_ARG(((uintptr_t)d_feat | (uintptr_t)d_h1 | (uintptr_t)d_h2) % 16 == 0 && (uintptr_t)d_rgb_half4 % 8 == 0, "misaligned buffer");
     RenderArgs a; memset(&a, 0, sizeof(a));
-    uint64_t n_entries = 0;
-    int rc = build_level_table(&args->grid, &a.lt, &n_entries); if (rc) return rc;
-    PERF_CHECK_SUP(args->grid.n_levels == 16, "fused field kernel needs n_levels == 16 (got %u)", args->grid.n_levels);
-    a.table = (const uint2*)args->d_packed_table;
-    PERF_CHECK_ARG((uintptr_t)args->d_packed_table % 16 == 0, "misaligned table");
-    const PackedLayout pl = packed_layout(a.lt, n_entries);
-    for (uint32_t l = 0; l < pl.n_cell_levels; ++l) a.cells[l] = reinterpret_cast<const uint4*>(a.table + pl.cell_start[l]);
-    a.geo_w = (const __half*)args->d_geo_mlp_half; a.app_w = (const __half*)args->d_app_mlp_half;
-    for (int i = 0; i < 3; ++i) { a.aabb_min[i] = args->aabb[i]; a.aabb_ext[i] = args->aabb[3 + i] - args->aabb[i]; }
-    set_div_mode(a);
+    bool fast = false;
+    int rc = init_field_args(args, a, fast); if (rc) return rc;
     a.rays_o = d_rays_o; a.rays_d = d_rays_d;
     a.s_feat = (uint4*)d_feat; a.s_h1 = (uint4*)d_h1; a.s_h2 = (uint4*)d_h2;
     if (N == 0) return PERF_OK;
@@ -1182,27 +1183,47 @@ static int fields_packed(const perf_render_args* args, const float* d_rays_o, co
     rc = prepare_weights(a, st); if (rc) return rc;
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
     const unsigned grid = (unsigned)(n_tiles < (uint64_t)num_sms() * 4 ? n_tiles : (uint64_t)num_sms() * 4);
-    const bool fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
-    // BYTES: RE_TOTAL for the eval kernels (phase 0), RS_TOTAL for the saving ones
-#define PERF_PACKED_LAUNCH(BYTES, ...) do { \
-        auto k = __VA_ARGS__; \
-        static thread_local int attr_dev = -1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_)); \
-        if (attr_dev != dev_) { const int rc_ = set_smem(k, BYTES, 4); if (rc_) return rc_; attr_dev = dev_; } \
-        k<<<grid, TILE, BYTES, st>>>(a, p); } while (0)
+    // bytes: RE_TOTAL for the eval kernels (phase 0), RE_TOTAL_N for their normals twins, RS_TOTAL for the saving ones
     if (p.normal != nullptr) {
-        if (fast) PERF_PACKED_LAUNCH(RE_TOTAL_N, packed_fields_kernel<4, 0, true>); else PERF_PACKED_LAUNCH(RE_TOTAL_N, packed_fields_kernel<-1, 0, true>);
+        rc = fast ? launch_field<packed_fields_kernel<4, 0, true>>(RE_TOTAL_N, grid, st, a, p) : launch_field<packed_fields_kernel<-1, 0, true>>(RE_TOTAL_N, grid, st, a, p);
     } else if (fast) {
-        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<4, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 1>);
-        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<4, 2>);
+        if (phase == 0) rc = launch_field<packed_fields_kernel<4, 0>>(RE_TOTAL, grid, st, a, p);
+        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<4, 1>>(RS_TOTAL, grid, st, a, p);
+        else rc = launch_field<packed_fields_kernel<4, 2>>(RS_TOTAL, grid, st, a, p);
     } else {
-        if (phase == 0) PERF_PACKED_LAUNCH(RE_TOTAL, packed_fields_kernel<-1, 0>);
-        else if (phase == PERF_PHASE_GEO) PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 1>);
-        else PERF_PACKED_LAUNCH(RS_TOTAL, packed_fields_kernel<-1, 2>);
+        if (phase == 0) rc = launch_field<packed_fields_kernel<-1, 0>>(RE_TOTAL, grid, st, a, p);
+        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<-1, 1>>(RS_TOTAL, grid, st, a, p);
+        else rc = launch_field<packed_fields_kernel<-1, 2>>(RS_TOTAL, grid, st, a, p);
     }
-#undef PERF_PACKED_LAUNCH
+    if (rc) return rc;
     PERF_LAUNCH_CHECK();
     return PERF_OK;
+}
+
+// perf_render_rays and perf_render_rays_normals (d_normal != null)
+static int render_rays(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && d_rays_o && d_rays_d, "NULL pointer");
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    a.rays_o = d_rays_o; a.rays_d = d_rays_d; a.R = R;
+    if (args->image_width > 0 && (args->flags & PERF_FLAG_SCAN_KERNEL) == 0) {
+        PERF_CHECK_ARG(R % args->image_width == 0, "image_width=%u does not divide the %llu rays", args->image_width, (unsigned long long)R);
+        a.W = (int)args->image_width;
+    }
+    a.normal = d_normal;
+    return launch_render(args, a, false, (cudaStream_t)stream, 0, d_normal != nullptr);
+}
+
+// perf_render_pano and perf_render_pano_normals (d_normal != null)
+static int render_pano(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && h_pose, "NULL pointer");
+    PERF_CHECK_ARG(H > 0 && W > 0 && row0 >= 0 && rows >= 0 && row0 + rows <= H, "bad panorama window H=%d W=%d row0=%d rows=%d", H, W, row0, rows);
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) a.pose_r[3 * r + c] = h_pose[4 * r + c]; a.pose_t[r] = h_pose[4 * r + 3]; }
+    a.H = H; a.W = W; a.row0 = row0; a.R = (uint64_t)rows * W;
+    a.normal = d_normal;
+    return launch_render(args, a, true, (cudaStream_t)stream, 0, d_normal != nullptr);
 }
 
 }  // namespace perf
@@ -1214,14 +1235,7 @@ extern "C" {
 
 int perf_render_rays(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R, void* stream)
 {
-    PERF_CHECK_ARG(args && d_rays_o && d_rays_d, "NULL pointer");
-    RenderArgs a; memset(&a, 0, sizeof(a));
-    a.rays_o = d_rays_o; a.rays_d = d_rays_d; a.R = R;
-    if (args->image_width > 0 && (args->flags & PERF_FLAG_SCAN_KERNEL) == 0) {
-        PERF_CHECK_ARG(R % args->image_width == 0, "image_width=%u does not divide the %llu rays", args->image_width, (unsigned long long)R);
-        a.W = (int)args->image_width;
-    }
-    return launch_render(args, a, false, (cudaStream_t)stream);
+    return render_rays(args, d_rays_o, d_rays_d, R, nullptr, stream);
 }
 
 int perf_render_packed(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R,
@@ -1272,12 +1286,7 @@ int perf_fields_packed(const perf_render_args* args, const float* d_rays_o, cons
 
 int perf_render_pano(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows, void* stream)
 {
-    PERF_CHECK_ARG(args && h_pose, "NULL pointer");
-    PERF_CHECK_ARG(H > 0 && W > 0 && row0 >= 0 && rows >= 0 && row0 + rows <= H, "bad panorama window H=%d W=%d row0=%d rows=%d", H, W, row0, rows);
-    RenderArgs a; memset(&a, 0, sizeof(a));
-    for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) a.pose_r[3 * r + c] = h_pose[4 * r + c]; a.pose_t[r] = h_pose[4 * r + 3]; }
-    a.H = H; a.W = W; a.row0 = row0; a.R = (uint64_t)rows * W;
-    return launch_render(args, a, true, (cudaStream_t)stream);
+    return render_pano(args, h_pose, H, W, row0, rows, nullptr, stream);
 }
 
 // ---- surface normals (perfb200.h: perf_render_pano_normals and the others)
@@ -1286,28 +1295,16 @@ int perf_render_pano(const perf_render_args* args, const float* h_pose, int H, i
 
 int perf_render_pano_normals(const perf_render_args* args, const float* h_pose, int H, int W, int row0, int rows, float* d_normal, void* stream)
 {
-    PERF_CHECK_ARG(args && h_pose && d_normal, "NULL pointer");
+    PERF_CHECK_ARG(args && d_normal, "NULL pointer");
     PERF_NORMALS_FLAGS_OK(args);
-    PERF_CHECK_ARG(H > 0 && W > 0 && row0 >= 0 && rows >= 0 && row0 + rows <= H, "bad panorama window H=%d W=%d row0=%d rows=%d", H, W, row0, rows);
-    RenderArgs a; memset(&a, 0, sizeof(a));
-    for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) a.pose_r[3 * r + c] = h_pose[4 * r + c]; a.pose_t[r] = h_pose[4 * r + 3]; }
-    a.H = H; a.W = W; a.row0 = row0; a.R = (uint64_t)rows * W;
-    a.normal = d_normal;
-    return launch_render(args, a, true, (cudaStream_t)stream, 0, true);
+    return render_pano(args, h_pose, H, W, row0, rows, d_normal, stream);
 }
 
 int perf_render_rays_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, uint64_t R, float* d_normal, void* stream)
 {
-    PERF_CHECK_ARG(args && d_rays_o && d_rays_d && d_normal, "NULL pointer");
+    PERF_CHECK_ARG(args && d_normal, "NULL pointer");
     PERF_NORMALS_FLAGS_OK(args);
-    RenderArgs a; memset(&a, 0, sizeof(a));
-    a.rays_o = d_rays_o; a.rays_d = d_rays_d; a.R = R;
-    if (args->image_width > 0) {
-        PERF_CHECK_ARG(R % args->image_width == 0, "image_width=%u does not divide the %llu rays", args->image_width, (unsigned long long)R);
-        a.W = (int)args->image_width;
-    }
-    a.normal = d_normal;
-    return launch_render(args, a, false, (cudaStream_t)stream, 0, true);
+    return render_rays(args, d_rays_o, d_rays_d, R, d_normal, stream);
 }
 
 int perf_fields_packed_normals(const perf_render_args* args, const float* d_rays_o, const float* d_rays_d, const int64_t* d_ray_indices,

@@ -23,7 +23,7 @@ template <int PHASE>
 __host__ __device__ __forceinline__ void composite_bwd_ray(const CompBwdArgs& a, uint64_t ray)
 {
     const uint32_t S = a.S;
-    const float step = PERF_FDIV_RN(PERF_FSUB_RN(a.far, a.near), (float)S);
+    const float step = fixed_s_step(a.near, a.far, S);
     const float jit = a.jitter ? a.jitter[ray] : 0.f;
     if constexpr (PHASE == PERF_PHASE_APP) {
         float gr = 0.f, gg = 0.f, gb = 0.f;
@@ -53,8 +53,7 @@ __host__ __device__ __forceinline__ void composite_bwd_ray(const CompBwdArgs& a,
             const uint64_t row = (uint64_t)kk * a.R + ray;
             const float toff = a.seg > 1 ? a.toff[(uint64_t)(kk / kps) * a.R + ray] : 1.f;     // segment-local -> global
             const float w = a.w[row] * toff, T = a.T[row] * toff, sig = a.sigma[row];
-            const float ts = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)kk, jit), step));
-            const float te = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)(kk + 1), jit), step));
+            const float ts = fixed_s_t(a.near, step, kk, jit), te = fixed_s_t(a.near, step, kk + 1, jit);
             const float m = PERF_FADD_RN(ts, te) * 0.5f, dt = PERF_FSUB_RN(te, ts);
             const float Wx = O - Wsuf - w, WMx = D - WMsuf - w * m;
             const float ddl = (2.f / 3.f) * dt * w + 2.f * (m * Wx - WMx) + 2.f * (WMsuf - m * Wsuf);
@@ -88,7 +87,7 @@ __global__ void __launch_bounds__(32 * C) composite_bwd_chunk_kernel(const CompB
     const bool valid = ray < a.R;
     const uint32_t S = a.S, K = S / C, k_lo = c * K, k_hi = k_lo + K;
     const uint32_t kps = S / a.seg;
-    const float step = __fdiv_rn(__fsub_rn(a.far, a.near), (float)S);
+    const float step = __fdiv_rn(__fsub_rn(a.far, a.near), (float)S);     // fixed_s_step, kept inline: calling it changes this kernel's registers
     const float jit = (valid && a.jitter) ? a.jitter[ray] : 0.f;
     if constexpr (PHASE == PERF_PHASE_APP) {
         if (!valid) return;
@@ -106,8 +105,7 @@ __global__ void __launch_bounds__(32 * C) composite_bwd_chunk_kernel(const CompB
     } else {
         __shared__ float sW[C][32], sWM[C][32], sWG[C][32];
         auto t_mid = [&](uint32_t k, float& m, float& dt) {
-            const float ts = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)k, jit), step));
-            const float te = __fadd_rn(a.near, __fmul_rn(__fadd_rn((float)(k + 1), jit), step));
+            const float ts = fixed_s_t(a.near, step, k, jit), te = fixed_s_t(a.near, step, k + 1, jit);
             m = __fadd_rn(ts, te) * 0.5f; dt = __fsub_rn(te, ts);
         };
         // pass 1: this chunk's sum w and sum w m
@@ -232,20 +230,20 @@ __host__ __device__ __forceinline__ void bwd_rays_row_level(const GridBwdRaysArg
     if (live) {
         g = *reinterpret_cast<const float2*>(a.dfeat + row * (2 * a.lt.n_levels) + 2 * l);
         const uint64_t ray = row % a.R; const uint32_t k = (uint32_t)(row / a.R);
-        const float step = PERF_FDIV_RN(PERF_FSUB_RN(a.far, a.near), (float)a.S);
+        const float step = fixed_s_step(a.near, a.far, a.S);
         const float jit = a.jitter ? a.jitter[ray] : 0.f;
-        const float ts = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)k, jit), step));
-        const float te = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)(k + 1), jit), step));
+        const float ts = fixed_s_t(a.near, step, k, jit), te = fixed_s_t(a.near, step, k + 1, jit);
         const float tsum = PERF_FADD_RN(ts, te);
-        x = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(a.rays_o[3 * ray], PERF_FMUL_RN(a.rays_d[3 * ray], tsum) * 0.5f), a.aabb_min[0]), a.aabb_ext[0]);
-        y = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(a.rays_o[3 * ray + 1], PERF_FMUL_RN(a.rays_d[3 * ray + 1], tsum) * 0.5f), a.aabb_min[1]), a.aabb_ext[1]);
-        z = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(a.rays_o[3 * ray + 2], PERF_FMUL_RN(a.rays_d[3 * ray + 2], tsum) * 0.5f), a.aabb_min[2]), a.aabb_ext[2]);
+        x = to_unit(sample_midpoint(a.rays_o[3 * ray], a.rays_d[3 * ray], tsum), a.aabb_min[0], a.aabb_ext[0]);
+        y = to_unit(sample_midpoint(a.rays_o[3 * ray + 1], a.rays_d[3 * ray + 1], tsum), a.aabb_min[1], a.aabb_ext[1]);
+        z = to_unit(sample_midpoint(a.rays_o[3 * ray + 2], a.rays_d[3 * ray + 2], tsum), a.aabb_min[2], a.aabb_ext[2]);
     }
     const bool active = live && (g.x != 0.f || g.y != 0.f);
     // level addressing with a dynamic level index (constant bank, uniform per block)
     const float scale = a.lt.scale[l];
     const uint32_t res = a.lt.res[l], size = a.lt.size[l], off = a.lt.offset[l];
     const bool hashed = (a.lt.hashed_mask >> l) & 1u, pow2 = (a.lt.pow2_mask >> l) & 1u;
+    // common.cuh::cell_frame, kept inline: calling it changes the register allocation of hashgrid_bwd_rays_kernel<false>
     const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
     const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
     const uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
@@ -284,7 +282,7 @@ __host__ __device__ __forceinline__ void bwd_march_ray_level(const GridBwdRaysAr
     // piece of the ray walked by this thread (more threads, shorter dependent loops; costs one extra flush per piece)
     const uint32_t k_per = (a.S + n_pieces - 1) / n_pieces;
     const uint32_t k_lo = piece * k_per, k_hi = a.S < k_lo + k_per ? a.S : k_lo + k_per;
-    const float step = PERF_FDIV_RN(PERF_FSUB_RN(a.far, a.near), (float)a.S);
+    const float step = fixed_s_step(a.near, a.far, a.S);
     const float jit = a.jitter ? a.jitter[ray] : 0.f;
     const float ox = a.rays_o[3 * ray], oy = a.rays_o[3 * ray + 1], oz = a.rays_o[3 * ray + 2];
     const float dx = a.rays_d[3 * ray], dy = a.rays_d[3 * ray + 1], dz = a.rays_d[3 * ray + 2];
@@ -321,12 +319,12 @@ __host__ __device__ __forceinline__ void bwd_march_ray_level(const GridBwdRaysAr
         const float2 g = a.plane_rows ? reinterpret_cast<const float2*>(a.dfeat)[(uint64_t)l * a.plane_rows + (uint64_t)ks * a.R + ray]
                                       : *reinterpret_cast<const float2*>(a.dfeat + ((uint64_t)ks * a.R + ray) * stride + 2 * l);
         if (g.x == 0.f && g.y == 0.f) continue;
-        const float ts = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)ks, jit), step));
-        const float te = PERF_FADD_RN(a.near, PERF_FMUL_RN(PERF_FADD_RN((float)(ks + 1), jit), step));
+        const float ts = fixed_s_t(a.near, step, ks, jit), te = fixed_s_t(a.near, step, ks + 1, jit);
         const float tsum = PERF_FADD_RN(ts, te);
-        const float x = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(ox, PERF_FMUL_RN(dx, tsum) * 0.5f), a.aabb_min[0]), a.aabb_ext[0]);
-        const float y = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(oy, PERF_FMUL_RN(dy, tsum) * 0.5f), a.aabb_min[1]), a.aabb_ext[1]);
-        const float z = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FADD_RN(oz, PERF_FMUL_RN(dz, tsum) * 0.5f), a.aabb_min[2]), a.aabb_ext[2]);
+        const float x = to_unit(sample_midpoint(ox, dx, tsum), a.aabb_min[0], a.aabb_ext[0]);
+        const float y = to_unit(sample_midpoint(oy, dy, tsum), a.aabb_min[1], a.aabb_ext[1]);
+        const float z = to_unit(sample_midpoint(oz, dz, tsum), a.aabb_min[2], a.aabb_ext[2]);
+        // common.cuh::cell_frame, split around the cell test: calling it changes the registers of hashgrid_bwd_march_kernel
         const float px = fmaf(scale, x, 0.5f), py = fmaf(scale, y, 0.5f), pz = fmaf(scale, z, 0.5f);
         const float fx = floorf(px), fy = floorf(py), fz = floorf(pz);
         const uint32_t gx = (uint32_t)(int)fx, gy = (uint32_t)(int)fy, gz = (uint32_t)(int)fz;
