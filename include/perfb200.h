@@ -68,7 +68,8 @@ typedef struct perf_mlp_cfg {
 #define PERF_FLAG_SIMT_MLP   2u   /* debug only: MLP on CUDA cores instead of wgmma       */
 #define PERF_FLAG_GENERIC_ADDR 8u  /* render: disable the specialised (4 dense + hashed pow2) addressing path */
 #define PERF_FLAG_L0_SMEM 16u      /* render_pano (experimental variant): level 0 of the table staged into
-                                      shared memory by one cp.async.bulk per CTA, fewer CTAs/SM */
+                                      shared memory by one cp.async.bulk per CTA and read by its four
+                                      warpgroups (the 132 KB shared-memory carveout instead of 100 KB) */
 #define PERF_FLAG_SCAN_KERNEL 4u   /* render: samples-along-lanes kernel (warp-shuffle scan composite) instead of ray marching */
 
 int         perf_abi_version(void);

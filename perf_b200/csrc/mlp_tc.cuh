@@ -1,6 +1,6 @@
 // mlp_tc.cuh -- building blocks of the 64-wide bias-free MLP on the Hopper tensor cores (wgmma).
 //
-// One CTA = 128 threads = one warpgroup = one 128-row tile; thread t owns row t: it produces the row's fp16 input
+// One warpgroup = 128 threads = one 128-row tile; thread t owns row t: it produces the row's fp16 input
 // features and runs the row's epilogue.  A layer is two M=64 wgmma chains (rows 0-63, 64-127) whose fp32 accumulator
 // fragments are rounded (ReLU, fp16) in registers and written straight into the next layer's operand image, from
 // which every thread then reads its own row back (layer_relu).  The eval renders skip that round trip after layer 1: the
@@ -28,6 +28,14 @@ constexpr int A32_BYTES = 4 * TILE * 16; //  8 KB : 128 x 32 fp16
 constexpr int A64_BYTES = 8 * TILE * 16; // 16 KB : 128 x 64 fp16
 constexpr int W32_BYTES = 4 * HID * 16;  //  4 KB :  64 x 32 fp16
 constexpr int W64_BYTES = 8 * HID * 16;  //  8 KB :  64 x 64 fp16
+
+// Barrier of this thread's warpgroup only (named barrier 1 + threadIdx.x / 128, 128 threads): the field kernels run up to
+// four independent 128-row tiles per CTA, one per warpgroup, and a tile's barriers must not wait for the others.  In a
+// 128-thread CTA it is equivalent to __syncthreads().
+__device__ __forceinline__ void wg_sync()
+{
+    asm volatile("bar.sync %0, 128;" :: "r"(1 + (int)(threadIdx.x >> 7)) : "memory");
+}
 
 // [64, K] row-major fp16 weights in global memory -> canonical K-major smem layout.
 __device__ __forceinline__ void load_weight_canonical(const __half* __restrict__ gW, int K, uint8_t* dst, int tid, int nthreads)
@@ -140,7 +148,7 @@ __device__ __forceinline__ void layer_relu(uint8_t* dst, const uint8_t* A, const
             simt_chunk(c, K, A, W, tid, v);
             relu_pack(v, hp[c]);
         }
-        if constexpr (OVERLAP) __syncthreads();
+        if constexpr (OVERLAP) wg_sync();
 #pragma unroll
         for (int c = 0; c < 2; ++c) store_chunk_canonical(dst, tid, 4 * c, hp[c]);
     } else {
@@ -158,7 +166,7 @@ __device__ __forceinline__ void layer_relu(uint8_t* dst, const uint8_t* A, const
                                 gmma_desc(smem_u32(W) + ks * 2 * W_LBO, W_LBO, X_SBO), ks > 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait();
-        if constexpr (OVERLAP) __syncthreads();
+        if constexpr (OVERLAP) wg_sync();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             uint8_t* const p = dst + (h * 64 + warp * 16 + (lane >> 2)) * 16 + (lane & 3) * 4;

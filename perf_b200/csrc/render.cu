@@ -65,59 +65,82 @@ struct RenderArgs {
     };
 };
 
-// Shared memory of the kernels that round-trip the hidden layers through shared memory: the training forward (SAVE = 1/2),
-// the SIMT twin and the legacy scan kernel.
-constexpr int RS_A     = 0;                         // 16 KB: A_geo | A_app, later the colour hidden layers (K=64)
-constexpr int RS_H     = RS_A + A64_BYTES;          // 16 KB: density hidden layer
-constexpr int RS_W1G   = RS_H + A64_BYTES;
-constexpr int RS_W1A   = RS_W1G + W32_BYTES;
-constexpr int RS_W2A   = RS_W1A + W32_BYTES;
-constexpr int RS_WOUT  = RS_W2A + W64_BYTES;        // 1 KB, unused (the output weights are read from c_wout)
-constexpr int RS_TAILS = RS_WOUT + 4 * HID * 4;     // [2 scans][4 warps][8] floats
-constexpr int RS_CARRY = RS_TAILS + 2 * 4 * 8 * 4;  // [2 parities][8] floats
-constexpr int RS_BARW  = RS_CARRY + 2 * 8 * 4;     // mbarrier of the weight bulk copy
-constexpr int RS_TOTAL = RS_BARW + 16;
+// Shared memory of a field kernel = one CTA-wide block (the weight operand images, staged once per CTA, and the mbarrier
+// of their bulk copy), then one region per warpgroup (WG_MAX of them at most, one 128-row tile each): the 4 tiles an SM
+// runs at a time read ONE copy of the weights, and what shared memory they do not use is L1 for the table gathers.
+// No warpgroup touches another warpgroup's region.
+constexpr int WG_MAX = 4;
+constexpr int align128(int b) { return (b + 127) / 128 * 128; }
 constexpr int W_IMG_BYTES = W32_BYTES + W32_BYTES + W64_BYTES;       // 16 KB: W1 density | W1 colour | W2 colour
-static_assert(RS_W1A == RS_W1G + W32_BYTES && RS_W2A == RS_W1A + W32_BYTES, "the three weight images are one contiguous block");
-
-// Shared memory of the eval kernels (wgmma MLP, no saves: eval_mlp_regs): the feature tile and the weight images only --
-// the hidden layers never leave the registers.  ~34 KB, so 4 CTAs fit the 164 KB shared-memory carveout and leave 92 KB
-// of the SM's 256 KB to the L1 that serves the table gathers (the layout above needs the 228 KB carveout: 28 KB of L1).
 constexpr int WO_BYTES = 8 * HID * 2;               // 1 KB: an output layer as an N = 8 operand image (mlp_tc.cuh layout, LBO = 128)
 constexpr int WO_LBO   = 8 * 16;
-constexpr int RE_A     = 0;                         // 16 KB: A_geo | A_app
-constexpr int RE_W1G   = RE_A + A64_BYTES;
+constexpr int W_IMG_ALL = W_IMG_BYTES + 2 * WO_BYTES;                // 18 KB: the hidden images, then the two output images
+
+// Kernels that round-trip the hidden layers through shared memory: the training forward (SAVE = 1/2), the SIMT twin and
+// the legacy scan kernel.  CTA-wide block:
+constexpr int RS_W1G   = 0;
+constexpr int RS_W1A   = RS_W1G + W32_BYTES;
+constexpr int RS_W2A   = RS_W1A + W32_BYTES;
+constexpr int RS_BARW  = RS_W2A + W64_BYTES;        // mbarrier of the weight bulk copy
+constexpr int RS_CTA   = align128(RS_BARW + 16);
+// ... per warpgroup:
+constexpr int RS_A     = 0;                         // 16 KB: A_geo | A_app, later the colour hidden layers (K=64)
+constexpr int RS_H     = RS_A + A64_BYTES;          // 16 KB: density hidden layer
+constexpr int RS_TAILS = RS_H + A64_BYTES;          // [2 scans][4 warps][8] floats
+constexpr int RS_CARRY = RS_TAILS + 2 * 4 * 8 * 4;  // [2 parities][8] floats
+constexpr int RS_WG    = align128(RS_CARRY + 2 * 8 * 4);
+static_assert(RS_W1A == RS_W1G + W32_BYTES && RS_W2A == RS_W1A + W32_BYTES, "the three weight images are one contiguous block");
+static_assert(RS_CTA + WG_MAX * RS_WG + 1024 <= 164 * 1024, "4 warpgroups (+1 KB reserved) fit the 164 KB shared-memory carveout");
+
+// Eval kernels (wgmma MLP, no saves: eval_mlp_regs): the hidden layers never leave the registers, so a warpgroup needs its
+// feature tile only.  CTA-wide block:
+constexpr int RE_W1G   = 0;
 constexpr int RE_W1A   = RE_W1G + W32_BYTES;
 constexpr int RE_W2A   = RE_W1A + W32_BYTES;
 constexpr int RE_WOG   = RE_W2A + W64_BYTES;        // density output row 0, rows 1-7 zero
 constexpr int RE_WOA   = RE_WOG + WO_BYTES;         // colour output rows 0-2, rows 3-7 zero
-constexpr int RE_MAX   = RE_WOA + WO_BYTES;         // [4 warps] longest packed ray (perf_render_packed)
-constexpr int RE_BARW  = RE_MAX + 16;               // mbarrier of the weight bulk copy
-constexpr int RE_TOTAL = RE_BARW + 16;
-constexpr int W_IMG_ALL = W_IMG_BYTES + 2 * WO_BYTES;                // 18 KB: the hidden images, then the two output images
+constexpr int RE_BARW  = RE_WOA + WO_BYTES;         // mbarrier of the weight bulk copy
+constexpr int RE_CTA   = align128(RE_BARW + 16);
 static_assert(RE_W1A == RE_W1G + W32_BYTES && RE_W2A == RE_W1A + W32_BYTES && RE_WOG == RE_W1G + W_IMG_BYTES &&
               RE_WOA == RE_WOG + WO_BYTES, "the five weight images are one contiguous block");
-static_assert(4 * (RE_TOTAL + 1024) <= 164 * 1024, "4 eval CTAs (+1 KB reserved each) fit the 164 KB shared-memory carveout");
+// ... per warpgroup:
+constexpr int RE_A     = 0;                         // 16 KB: A_geo | A_app
+constexpr int RE_MAX   = RE_A + A64_BYTES;          // [4 warps] longest packed ray (perf_render_packed)
+constexpr int RE_WG    = align128(RE_MAX + 16);
+static_assert(RE_CTA + WG_MAX * RE_WG + 1024 <= 100 * 1024, "4 eval warpgroups (+1 KB reserved) fit the 100 KB shared-memory carveout");
 // The normals kernels (NORMAL) append per thread the sample position and the ray's running sum w n: the layer-1 peak of
 // the MLP leaves no register for them (the eval march kernel uses all 128 without them).
-constexpr int RE_XYZ   = (RE_TOTAL + 15) / 16 * 16;    // float4 [128]: x01, selector
-constexpr int RE_NACC  = RE_XYZ + TILE * 16;            // float4 [128]: sum w n of the thread's ray (march kernel)
-constexpr int RE_TOTAL_N = RE_NACC + TILE * 16;
-static_assert(4 * (RE_TOTAL_N + 1024) <= 164 * 1024, "4 normals CTAs fit the 164 KB shared-memory carveout");
-// measurement hook (tools/ab_lib.py): extra, unused dynamic shared memory per CTA of the march kernels, i.e. what
+constexpr int RE_XYZ   = RE_MAX + 16;               // float4 [128]: x01, selector
+constexpr int RE_NACC  = RE_XYZ + TILE * 16;        // float [3][128]: sum w n of the thread's ray (march kernel)
+constexpr int RE_WG_N  = align128(RE_NACC + 3 * TILE * 4);
+static_assert(RE_CTA + WG_MAX * RE_WG_N + 1024 <= 100 * 1024, "4 normals warpgroups fit the 100 KB shared-memory carveout");
+// experiment (PERF_FLAG_L0_SMEM, eval layout): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared
+// memory behind the weights, staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an
+// mbarrier) and read by all its warpgroups
+constexpr int RE_BAR2  = RE_CTA;
+constexpr int RE_L0    = RE_BAR2 + 128;
+constexpr int L0_BYTES = 4096 * 8;
+constexpr int RE_CTA_L0 = RE_L0 + L0_BYTES;
+// measurement hook (tools/ab_lib.py): extra, unused dynamic shared memory per warpgroup of the field kernels, i.e. what
 // more shared memory would cost in L1 capacity
 #ifndef PERF_RS_PAD
 #define PERF_RS_PAD 0
 #endif
-constexpr int RS_LAUNCH = RS_TOTAL + PERF_RS_PAD;
-constexpr int RE_LAUNCH = RE_TOTAL + PERF_RS_PAD;
-constexpr int RE_LAUNCH_N = RE_TOTAL_N + PERF_RS_PAD;
-// experiment (PERF_FLAG_L0_SMEM, eval layout): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared
-// memory, staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an mbarrier)
-constexpr int RE_BAR2  = (RE_TOTAL + 127) / 128 * 128;
-constexpr int RE_L0    = RE_BAR2 + 128;
-constexpr int L0_BYTES = 4096 * 8;
-constexpr int RE_TOTAL_L0 = RE_L0 + L0_BYTES;
+
+// Bytes the carveout percentage set_smem requests stands for on the H100 (228 KB of shared memory per SM at most): the
+// driver takes the next supported carveout at or above it, so a layout meant for a given carveout must keep this under it.
+constexpr long long carveout_request(long long need) { return (100 * need + 233471) / 233472 * 233472 / 100; }
+static_assert(carveout_request(RS_CTA + WG_MAX * RS_WG + 1024) <= 164 * 1024, "RS layout: the 164 KB carveout");
+static_assert(carveout_request(RE_CTA + WG_MAX * RE_WG + 1024) <= 100 * 1024, "eval layout: the 100 KB carveout");
+static_assert(carveout_request(RE_CTA + WG_MAX * RE_WG_N + 1024) <= 100 * 1024, "normals layout: the 100 KB carveout");
+static_assert(carveout_request(RE_CTA_L0 + WG_MAX * RE_WG + 1024) <= 132 * 1024, "level-0 layout: the 132 KB carveout");
+
+// Shared-memory shape of a field kernel: the CTA-wide block, then `nwg` regions of `wg_bytes`.
+struct FieldSmem {
+    int cta_bytes, wg_bytes;
+    int bytes(int nwg) const { return cta_bytes + nwg * (wg_bytes + PERF_RS_PAD); }
+};
+constexpr FieldSmem RS_SMEM = {RS_CTA, RS_WG}, RE_SMEM = {RE_CTA, RE_WG}, RE_SMEM_N = {RE_CTA, RE_WG_N}, RE_SMEM_L0 = {RE_CTA_L0, RE_WG};
 
 // Output-layer weights of both networks as fp32 in the CONSTANT bank: [0,64) density row, [64,256) the three colour
 // rows.  The 64 * n_out FMAs per sample of the output layers then take their weight operand straight from c[bank][imm]
@@ -149,14 +172,14 @@ __global__ void __launch_bounds__(1024) weights_prepare_kernel(const __half* __r
     }
 }
 
-// all threads of the CTA: weight images global -> shared memory by one bulk copy; returns when they have landed.
-// EVAL: the eval layout (RE_*, all five images); otherwise RS_* and the three hidden-layer images.
+// all threads of the CTA: weight images global -> the CTA-wide block of shared memory by one bulk copy; returns when they
+// have landed.  EVAL: the eval layout (RE_*, all five images); otherwise RS_* and the three hidden-layer images.
 template <bool EVAL>
-__device__ __forceinline__ void stage_weights_bulk(uint8_t* smem, int tid)
+__device__ __forceinline__ void stage_weights_bulk(uint8_t* smem)
 {
     constexpr int bytes = EVAL ? W_IMG_ALL : W_IMG_BYTES;
     uint64_t* barw = reinterpret_cast<uint64_t*>(smem + (EVAL ? RE_BARW : RS_BARW));
-    if (tid == 0) {
+    if (threadIdx.x == 0) {
         mbar_init(barw, 1); fence_mbar_init();
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(barw)), "r"(bytes) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -243,7 +266,7 @@ __device__ __forceinline__ void ray_scan(float (&val)[NV], float (&excl)[NV], ui
     }
 }
 
-// Pixel-patch tiling of a 128-thread tile: a warp covers PATCH_WW x PATCH_WH pixels, the CTA's four
+// Pixel-patch tiling of a 128-thread tile: a warp covers PATCH_WW x PATCH_WH pixels, the tile's four
 // warps are arranged PATCH_WX x PATCH_WY.
 #ifndef PATCH_WW
 #define PATCH_WW 8
@@ -396,7 +419,7 @@ __device__ __forceinline__ void eval_mlp_regs(const RenderSmem& sm, int lane, fl
             relu_frag(dg, hg);
             relu_frag(da, ha);
         }
-        if (h == 1) __syncthreads();                        // no warp reads the feature tiles any more
+        if (h == 1) wg_sync();                              // no warp reads the feature tiles any more
         float d2[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) d2[i] = 0.f;
@@ -464,7 +487,7 @@ __device__ __forceinline__ void eval_density_g(const RenderSmem& sm, int tid)
         for (int i = 0; i < 32; ++i) m |= (dg[i] > 0.f ? 1u : 0u) << i;
         gm[h] = m;
     }
-    __syncthreads();                                         // no warp reads the feature tiles any more: g may overwrite them
+    wg_sync();                                               // no warp reads the feature tiles any more: g may overwrite them
     uint32_t wo[8];                                          // w_out columns 8j + 2q, +1 (fp16 pair; output image row 0)
 #pragma unroll
     for (int j = 0; j < 8; ++j) wo[j] = *reinterpret_cast<const uint32_t*>(sm.sWog + j * 128 + q * 4);
@@ -557,11 +580,11 @@ __device__ __forceinline__ void sample_normal(const RenderArgs& a, const RenderS
     n[0] = -gx * r; n[1] = -gy * r; n[2] = -gz * r;
 }
 
-// Encode + both MLPs for the CTA's current 128 samples (thread t = one sample at normalised position (x,y,z)); all
-// 128 threads call it.
+// Encode + both MLPs for the warpgroup's current 128 samples (thread t = one sample at normalised position (x,y,z)); all
+// 128 threads of the warpgroup call it, and its barriers (wg_sync) wait for those 128 only.
 // EVAL (eval kernels: SIMT = false, SAVE = 0, eval shared-memory layout): hidden layers in registers (eval_mlp_regs), two
-// block-wide barriers.  Otherwise thread t owns row t of the tiles, every layer goes through shared memory and the output
-// layers run on CUDA cores (out_dots_const); 5 block-wide barriers.
+// barriers.  Otherwise thread t owns row t of the tiles, every layer goes through shared memory and the output
+// layers run on CUDA cores (out_dots_const); 5 barriers.
 // NDENSE >= 0: specialised addressing (level_corners_fast; first NDENSE levels dense, rest hashed
 // power-of-two) -- branch-free and ~1/3 smaller code; NDENSE < 0: generic addressing.
 // SAVE 1 / 2: also write the fp16 features and hidden activations of the density / colour network
@@ -596,7 +619,7 @@ __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSme
 
     if constexpr (EVAL) {
         fence_proxy_async();                                  // the feature tiles are the operand of layer 1
-        __syncthreads();
+        wg_sync();
         float lg, lr, lgr, lb;
         eval_mlp_regs(sm, tid & 31, lg, lr, lgr, lb);
         if constexpr (NORMAL) {
@@ -616,11 +639,11 @@ __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSme
 
     // ---- layer 1 of both nets: density hidden -> H, colour hidden 1 -> A (over the feature tiles)
     if constexpr (!SIMT) fence_proxy_async();
-    __syncthreads();
+    wg_sync();
     layer_relu<SIMT>(sH, sAg, sW1g, 32, tid);
     layer_relu<SIMT, true>(sA, sAa, sW1a, 32, tid);
     if constexpr (!SIMT) fence_proxy_async();             // A is the operand of the colour layer 2
-    __syncthreads();
+    wg_sync();
 
     // density: ReLU hidden -> 64-long dot -> fp16 logit -> exp     (ngp_nerf.py:141-150)
     float2 og[1] = {make_float2(0.f, 0.f)};
@@ -641,7 +664,7 @@ __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSme
     }
     // ---- colour layer 2, in place
     layer_relu<SIMT, true>(sA, sA, sW2a, 64, tid);
-    __syncthreads();
+    wg_sync();
     float2 oa[3] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
@@ -659,20 +682,21 @@ template <bool PANO, bool SIMT>
 __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__ RenderArgs a)
 {
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sA   = smem + RS_A;
+    uint8_t* const wgs = smem + RS_CTA;     // the one warpgroup's region
+    uint8_t* sA   = wgs + RS_A;
     uint8_t* sAg  = sA;                     // geo features, K=32
     uint8_t* sAa  = sA + A32_BYTES;         // app features, K=32
-    uint8_t* sH   = smem + RS_H;
+    uint8_t* sH   = wgs + RS_H;
     uint8_t* sW1g = smem + RS_W1G;
     uint8_t* sW1a = smem + RS_W1A;
     uint8_t* sW2a = smem + RS_W2A;
-    float*   sTails = reinterpret_cast<float*>(smem + RS_TAILS);
-    float*   sCarry = reinterpret_cast<float*>(smem + RS_CARRY);
+    float*   sTails = reinterpret_cast<float*>(wgs + RS_TAILS);
+    float*   sCarry = reinterpret_cast<float*>(wgs + RS_CARRY);
 
     const int tid = threadIdx.x;
     const RenderSmem sm = {sA, sAg, sAa, sH, sW1g, sW1a, sW2a, nullptr, nullptr, nullptr};
 
-    stage_weights_bulk<false>(smem, tid);            // W1 density | W1 colour | W2 colour operand images, one bulk copy
+    stage_weights_bulk<false>(smem);                 // W1 density | W1 colour | W2 colour operand images, one bulk copy
 
     const uint32_t S = a.S;
     const float step = fixed_s_step(a.near, a.far, S);
@@ -765,24 +789,31 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
 // (temporal L1 reuse).  The composite is a per-thread running sum: no shuffles, no carries.
 // Transmittance uses the sequential exclusive sum, the order of the oracle's cumsum.
 // NORMAL: also a.normal[ray] = sum_i w_i n_i (eval layout, seg == 1).
+// A CTA is blockDim.x / 128 warpgroups (launch_field), each an independent tile loop over its own shared-memory region:
+// warpgroup wg of CTA b takes work items b * nwg + wg, b * nwg + wg + gridDim.x * nwg, ...
 template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false, bool NORMAL = false>
-__global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(const __grid_constant__ RenderArgs a)
+__global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __grid_constant__ RenderArgs a)
 {
     constexpr bool EVAL = !SIMT && SAVE == 0;        // hidden layers in registers, eval shared-memory layout (RE_*)
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sA   = smem + (EVAL ? RE_A : RS_A);
+    // wg broadcast from lane 0: the compiler then knows it is warp-uniform and keeps the region's address and the wgmma
+    // descriptors built from it in uniform registers (threadIdx.x / TILE alone costs the 128-register kernels spills)
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x / TILE, 0), nwg = blockDim.x / TILE;
+    uint8_t* const wgs = smem + (EVAL ? (L0SMEM ? RE_CTA_L0 : RE_CTA) + wg * (NORMAL ? RE_WG_N : RE_WG) : RS_CTA + wg * RS_WG) +
+                         wg * PERF_RS_PAD;       // this warpgroup's region
+    uint8_t* sA   = wgs + (EVAL ? RE_A : RS_A);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = NORMAL ? (int)(threadIdx.x % TILE) : (int)threadIdx.x - wg * TILE, warp = tid >> 5, lane = tid & 31;
     const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
                                             smem + RE_WOA, L0SMEM ? reinterpret_cast<const uint2*>(smem + RE_L0) : nullptr,
-                                            NORMAL ? reinterpret_cast<float4*>(smem + RE_XYZ) : nullptr}
-                               : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
+                                            NORMAL ? reinterpret_cast<float4*>(wgs + RE_XYZ) : nullptr}
+                               : RenderSmem{sA, sA, sA + A32_BYTES, wgs + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
                                             nullptr, nullptr};
 
-    stage_weights_bulk<EVAL>(smem, tid);             // the weight operand images, one bulk copy
+    stage_weights_bulk<EVAL>(smem);                  // the weight operand images, one bulk copy
     if constexpr (L0SMEM) {
         uint64_t* bar2 = reinterpret_cast<uint64_t*>(smem + RE_BAR2);
-        if (tid == 0) {
+        if (threadIdx.x == 0) {
             mbar_init(bar2, 1); fence_mbar_init();
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar2)), "r"(L0_BYTES) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -806,11 +837,17 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
     const uint32_t my_seg = (uint32_t)tid / rpt;
     const uint64_t n_tiles = patch ? (uint64_t)tiles_x * (uint64_t)patch_rows(rows) : (a.R + rpt - 1) / rpt;
 
-    for (uint64_t work = blockIdx.x; work < n_tiles; work += gridDim.x) {
+    // Work items of this warpgroup: blockIdx.x * nwg + wg, then steps of gridDim.x * nwg (n_tiles < 2^31, launch_render).
+    // The normals kernels add wg inside the loop instead of into its start, and take tid from threadIdx.x % TILE: the same
+    // values, but ptxas allocates the two forms differently, and each form is the one that keeps its kernels' spills
+    // within what they were with one warpgroup per CTA (the others spill in the 128-register kernels).
+    constexpr uint32_t wg_in_start = NORMAL ? 0u : 1u;
+    for (uint32_t w0 = blockIdx.x * nwg + wg * wg_in_start; w0 + wg * (1u - wg_in_start) < n_tiles; w0 += gridDim.x * nwg) {
+        const uint32_t work = w0 + wg * (1u - wg_in_start);
         // Image-shaped work is dealt out in a scattered order: the tiles in flight at any moment (4 per SM) are spread over
         // the whole image instead of forming one band of neighbouring tiles that all pull the same table lines through the
         // same L2 slices at the same time.
-        const uint64_t tile = (patch && a.tile_mul > 1u) ? (work * a.tile_mul) % n_tiles : work;
+        const uint64_t tile = (patch && a.tile_mul > 1u) ? ((uint64_t)work * a.tile_mul) % n_tiles : work;
         // ---- this thread's ray
         uint64_t ray; bool valid;
         float ox = 0.f, oy = 0.f, oz = 0.f, dx = 1.f, dy = 0.f, dz = 0.f, jit = 0.f;
@@ -851,8 +888,8 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
         float sum_sd = 0.f;                                   // exclusive running sum of sigma*dt
         float acc_w = 0.f, acc_d = 0.f, acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;
         float dl_uni = 0.f, dl_bi = 0.f;                      // distortion loss pieces (SAVE only)
-        float4* const acc_n = reinterpret_cast<float4*>(smem + RE_NACC) + tid;     // sum w n (NORMAL only)
-        if constexpr (NORMAL) *acc_n = make_float4(0.f, 0.f, 0.f, 0.f);
+        float* const acc_n = reinterpret_cast<float*>(wgs + RE_NACC) + tid;        // sum w n (NORMAL only): [3][128]
+        if constexpr (NORMAL) { acc_n[0] = 0.f; acc_n[TILE] = 0.f; acc_n[2 * TILE] = 0.f; }
         // packed mode: every thread walks ITS ray's samples; the tile iterates to the longest ray
         // (neighbouring rays cross the same occupied shells, so lengths inside a tile are similar)
         uint32_t n_iter = kps, my_count = S;
@@ -861,10 +898,10 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             my_count = 0;
             if (valid) { pk_base = a.pk_offsets[ray]; my_count = (uint32_t)(a.pk_offsets[ray + 1] - pk_base); }
             const uint32_t wmax = __reduce_max_sync(0xffffffffu, my_count);
-            uint32_t* s_max = reinterpret_cast<uint32_t*>(smem + (EVAL ? RE_MAX : RS_TAILS));
-            __syncthreads();                                  // previous tile's readers are done
+            uint32_t* s_max = reinterpret_cast<uint32_t*>(wgs + (EVAL ? RE_MAX : RS_TAILS));
+            wg_sync();                                        // previous tile's readers are done
             if (lane == 0) s_max[warp] = wmax;
-            __syncthreads();
+            wg_sync();
             n_iter = max(max(s_max[0], s_max[1]), max(s_max[2], s_max[3]));
         }
 #pragma unroll 1
@@ -909,11 +946,11 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             acc_w += w; acc_d = fmaf(w, tsum * 0.5f, acc_d);
             acc_r = fmaf(w, cr, acc_r); acc_g = fmaf(w, cg, acc_g); acc_b = fmaf(w, cb, acc_b);
             if constexpr (NORMAL) {
-                float4 an = *acc_n;
+                float3 an = make_float3(acc_n[0], acc_n[TILE], acc_n[2 * TILE]);
                 an.x = fmaf(w, nrm[0], an.x); an.y = fmaf(w, nrm[1], an.y); an.z = fmaf(w, nrm[2], an.z);
-                *acc_n = an;
+                acc_n[0] = an.x; acc_n[TILE] = an.y; acc_n[2 * TILE] = an.z;
             }
-            if constexpr (SIMT) __syncthreads();
+            if constexpr (SIMT) wg_sync();
         }
 
         bool writer = valid;
@@ -921,11 +958,11 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             // combine the `seg` partial composites of every ray (each computed as if T = 1 at the segment
             // start): w = Toff w', Wx = Wpre + Toff Wx', ... ; scratch = the (now idle) feature tiles
             float* part = reinterpret_cast<float*>(sA);
-            __syncthreads();
+            wg_sync();
             part[0 * TILE + tid] = sum_sd; part[1 * TILE + tid] = acc_w; part[2 * TILE + tid] = acc_d;
             part[3 * TILE + tid] = acc_r;  part[4 * TILE + tid] = acc_g; part[5 * TILE + tid] = acc_b;
             part[6 * TILE + tid] = dl_uni; part[7 * TILE + tid] = dl_bi;
-            __syncthreads();
+            wg_sync();
             writer = valid && my_seg == 0;
             if (writer) {
                 float cum_sd = 0.f, W = 0.f, D = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, du = 0.f, db = 0.f;
@@ -942,7 +979,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
                 }
                 acc_w = W; acc_d = D; acc_r = cr; acc_g = cg; acc_b = cb; dl_uni = du; dl_bi = db;
             }
-            __syncthreads();                                      // scratch is rewritten by the next tile's features
+            wg_sync();                                            // scratch is rewritten by the next tile's features
         }
         if (writer) {
             const float one_m = 1.f - acc_w;
@@ -961,7 +998,7 @@ __global__ void __launch_bounds__(TILE, L0SMEM ? 2 : 4) render_march_kernel(cons
             a.rgb[3 * ray] = r; a.rgb[3 * ray + 1] = g; a.rgb[3 * ray + 2] = b;
             a.distance[ray] = dist;
             if (a.opacity) a.opacity[ray] = acc_w;
-            if constexpr (NORMAL) { const float4 an = *acc_n; a.normal[3 * ray] = an.x; a.normal[3 * ray + 1] = an.y; a.normal[3 * ray + 2] = an.z; }
+            if constexpr (NORMAL) { a.normal[3 * ray] = acc_n[0]; a.normal[3 * ray + 1] = acc_n[TILE]; a.normal[3 * ray + 2] = acc_n[2 * TILE]; }
         }
     }
 }
@@ -984,23 +1021,26 @@ struct PackedFieldArgs {
     float*         normal;        // [N,3] sample normals (NORMAL kernels)
 };
 
+// A CTA is blockDim.x / 128 warpgroups with one tile loop each, as in render_march_kernel.
 template <int NDENSE, int SAVE, bool NORMAL = false>
-__global__ void __launch_bounds__(TILE, 4) packed_fields_kernel(const __grid_constant__ RenderArgs a, const PackedFieldArgs p)
+__global__ void __launch_bounds__(WG_MAX * TILE, 1) packed_fields_kernel(const __grid_constant__ RenderArgs a, const PackedFieldArgs p)
 {
     constexpr bool EVAL = SAVE == 0;                 // hidden layers in registers, eval shared-memory layout (RE_*)
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sA   = smem + (EVAL ? RE_A : RS_A);
-    const int tid = threadIdx.x;
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x / TILE, 0), nwg = blockDim.x / TILE;   // warp-uniform: see render_march_kernel
+    uint8_t* const wgs = smem + (EVAL ? RE_CTA + wg * (NORMAL ? RE_WG_N : RE_WG) : RS_CTA + wg * RS_WG) + wg * PERF_RS_PAD;
+    uint8_t* sA   = wgs + (EVAL ? RE_A : RS_A);
+    const int tid = threadIdx.x % TILE;
     const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
-                                            smem + RE_WOA, nullptr, NORMAL ? reinterpret_cast<float4*>(smem + RE_XYZ) : nullptr}
-                               : RenderSmem{sA, sA, sA + A32_BYTES, smem + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
+                                            smem + RE_WOA, nullptr, NORMAL ? reinterpret_cast<float4*>(wgs + RE_XYZ) : nullptr}
+                               : RenderSmem{sA, sA, sA + A32_BYTES, wgs + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
                                             nullptr, nullptr};
-    stage_weights_bulk<EVAL>(smem, tid);             // the weight operand images, one bulk copy
+    stage_weights_bulk<EVAL>(smem);                  // the weight operand images, one bulk copy
     uint64_t N = p.N;
     if (p.n_dev) { const int64_t nd = *p.n_dev; N = nd < 0 ? 0 : ((uint64_t)nd < N ? (uint64_t)nd : N); }      // graph-replayable count
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
     const float rext0 = __frcp_rn(a.aabb_ext[0]), rext1 = __frcp_rn(a.aabb_ext[1]), rext2 = __frcp_rn(a.aabb_ext[2]);
-    for (uint64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    for (uint64_t tile = (uint64_t)blockIdx.x * nwg + wg; tile < n_tiles; tile += (uint64_t)gridDim.x * nwg) {
         const uint64_t n = tile * TILE + tid;
         const bool valid = n < N;
         float x = 0.5f, y = 0.5f, z = 0.5f;
@@ -1042,8 +1082,8 @@ static uint32_t gcd_u32(uint32_t a, uint32_t b) { while (b) { uint32_t t = a % b
 
 // Dynamic shared memory of a field kernel and its shared-memory carveout: the smallest that holds `ctas` resident CTAs (the
 // driver rounds the percentage up to the next size the SM supports), so that the rest of the SM's unified L1 / shared
-// memory stays L1 for the table gathers.  Not left to the driver's default: the eval layout (4 x 35 KB) fits the 164 KB
-// carveout, which leaves 92 KB of L1 where the 228 KB one leaves 28 KB.
+// memory stays L1 for the table gathers.  Not left to the driver's default: the eval layout (4 warpgroups, 84.6 KB) fits the
+// 100 KB carveout, which leaves 156 KB of L1 where the 228 KB one leaves 28 KB.
 template <typename K>
 static int set_smem(K k, int bytes, int ctas)
 {
@@ -1059,14 +1099,30 @@ static int set_smem(K k, int bytes, int ctas)
     return PERF_OK;
 }
 
-// Launch of field kernel K with `bytes` of dynamic shared memory; set_smem (4 CTAs / SM) runs once per device and kernel.
+// Launch of field kernel K over n_work 128-row tiles, WG_MAX tiles in flight per SM.  nwg_max = WG_MAX (render_march_kernel,
+// packed_fields_kernel): one CTA per SM of nwg = clamp(ceil(n_work / SMs), 1, WG_MAX) warpgroups that share one copy of the
+// weights, so a small launch still spreads one tile per SM.  nwg_max = 1 (the legacy scan kernel): WG_MAX 128-thread CTAs
+// per SM.  Once per device and kernel: the carveout for the nwg_max shape (set_smem), and a check that it is resident.
 template <auto K, class... P>
-static int launch_field(int bytes, unsigned grid, cudaStream_t stream, const P&... p)
+static int launch_field(const FieldSmem& fs, int nwg_max, uint64_t n_work, cudaStream_t stream, const P&... p)
 {
     static thread_local int attr_dev = -1;
+    const int ctas_per_sm = WG_MAX / nwg_max;
     int dev = 0; PERF_CUDA(cudaGetDevice(&dev));
-    if (attr_dev != dev) { const int rc = set_smem(K, bytes, 4); if (rc) return rc; attr_dev = dev; }
-    K<<<grid, TILE, bytes, stream>>>(p...);
+    if (attr_dev != dev) {
+        const int rc = set_smem(K, fs.bytes(nwg_max), ctas_per_sm); if (rc) return rc;
+        int resident = 0;
+        PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, K, nwg_max * TILE, fs.bytes(nwg_max)));
+        PERF_CHECK_SUP(resident >= ctas_per_sm, "field kernel: %d CTAs of %d threads and %d B of shared memory per SM, %d resident",
+                       ctas_per_sm, nwg_max * TILE, fs.bytes(nwg_max), resident);
+        attr_dev = dev;
+    }
+    const uint64_t ctas = (uint64_t)num_sms() * ctas_per_sm;
+    const uint64_t want = (n_work + ctas - 1) / ctas;
+    const int nwg = want < (uint64_t)nwg_max ? (int)want : nwg_max;
+    const uint64_t need = (n_work + nwg - 1) / nwg;
+    const unsigned grid = (unsigned)(need < ctas ? need : ctas);
+    K<<<grid, nwg * TILE, fs.bytes(nwg), stream>>>(p...);
     return PERF_OK;
 }
 
@@ -1120,43 +1176,34 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         const uint32_t rpt = TILE / (a.seg ? a.seg : 1u);
         n_work = (a.R + rpt - 1) / rpt;
     }
-    const unsigned grid = (unsigned)(n_work < (uint64_t)num_sms() * 4 ? n_work : (uint64_t)num_sms() * 4);
+    PERF_CHECK_SUP(n_work < (1ull << 31), "%llu tiles of 128 rays in one launch (at most 2^31)", (unsigned long long)n_work);
     a.tile_mul = 0;
-    if (PERF_TILE_SCATTER && !scan && (pano || a.W > 0) && n_work > grid && n_work < (1ull << 31)) {
+    if (PERF_TILE_SCATTER && !scan && (pano || a.W > 0) && n_work > (uint64_t)num_sms() * WG_MAX && n_work < (1ull << 31)) {
         // golden-ratio stride, made coprime with the tile count: consecutive work items land far apart, evenly spread
         uint32_t m = (uint32_t)((double)n_work * 0.6180339887498949) | 1u;
         while (m > 1u && gcd_u32(m, (uint32_t)n_work) != 1u) m += 2u;
         a.tile_mul = m % (uint32_t)n_work;
     }
     rc = prepare_weights(a, stream); if (rc) return rc;     // constant-bank output weights + operand images (c_wout, g_wimg)
-    // bytes: RE_LAUNCH for the eval kernels (SIMT = false, SAVE = 0), RE_LAUNCH_N for their normals twins, RS_LAUNCH for the others
+    // shared memory: RE_SMEM for the eval kernels (SIMT = false, SAVE = 0), RE_SMEM_N for their normals twins, RS_SMEM for the others
     if (normals) {                                                // surface normals: eval march kernel only (the callers refuse the rest)
-        if (fast) rc = pano ? launch_field<render_march_kernel<true, false, 4, 0, false, true>>(RE_LAUNCH_N, grid, stream, a) : launch_field<render_march_kernel<false, false, 4, 0, false, true>>(RE_LAUNCH_N, grid, stream, a);
-        else      rc = pano ? launch_field<render_march_kernel<true, false, -1, 0, false, true>>(RE_LAUNCH_N, grid, stream, a) : launch_field<render_march_kernel<false, false, -1, 0, false, true>>(RE_LAUNCH_N, grid, stream, a);
+        if (fast) rc = pano ? launch_field<render_march_kernel<true, false, 4, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a);
+        else      rc = pano ? launch_field<render_march_kernel<true, false, -1, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a);
     } else if (save != 0) {
         PERF_CHECK_SUP(!pano && !simt && !scan, "training forward runs on the ray-marching tensor-core kernel only");
-        if (fast) rc = save == 1 ? launch_field<render_march_kernel<false, false, 4, 1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, 4, 2>>(RS_LAUNCH, grid, stream, a);
-        else      rc = save == 1 ? launch_field<render_march_kernel<false, false, -1, 1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, -1, 2>>(RS_LAUNCH, grid, stream, a);
-    } else if (scan) {
-        if (pano) rc = simt ? launch_field<render_kernel<true, true>>(RS_LAUNCH, grid, stream, a) : launch_field<render_kernel<true, false>>(RS_LAUNCH, grid, stream, a);
-        else      rc = simt ? launch_field<render_kernel<false, true>>(RS_LAUNCH, grid, stream, a) : launch_field<render_kernel<false, false>>(RS_LAUNCH, grid, stream, a);
+        if (fast) rc = save == 1 ? launch_field<render_march_kernel<false, false, 4, 1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4, 2>>(RS_SMEM, WG_MAX, n_work, stream, a);
+        else      rc = save == 1 ? launch_field<render_march_kernel<false, false, -1, 1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1, 2>>(RS_SMEM, WG_MAX, n_work, stream, a);
+    } else if (scan) {                                            // legacy scan kernel: 128-thread CTAs
+        if (pano) rc = simt ? launch_field<render_kernel<true, true>>(RS_SMEM, 1, n_work, stream, a) : launch_field<render_kernel<true, false>>(RS_SMEM, 1, n_work, stream, a);
+        else      rc = simt ? launch_field<render_kernel<false, true>>(RS_SMEM, 1, n_work, stream, a) : launch_field<render_kernel<false, false>>(RS_SMEM, 1, n_work, stream, a);
     } else if (simt) {
-        rc = pano ? launch_field<render_march_kernel<true, true, -1>>(RS_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, true, -1>>(RS_LAUNCH, grid, stream, a);
-    } else if (fast && pano && (args->flags & PERF_FLAG_L0_SMEM)) {
-        auto k = render_march_kernel<true, false, 4, 0, true>;           // experiment: level 0 in shared memory (2 CTAs/SM)
-        static thread_local int attr_dev0 = -1, per_sm0 = 1; int dev_ = 0; PERF_CUDA(cudaGetDevice(&dev_));
-        if (attr_dev0 != dev_) {
-            rc = set_smem(k, RE_TOTAL_L0, 2); if (rc) return rc;
-            PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm0, k, TILE, RE_TOTAL_L0));
-            if (per_sm0 < 1) per_sm0 = 1;
-            attr_dev0 = dev_;
-        }
-        const uint64_t slots0 = (uint64_t)num_sms() * (uint64_t)per_sm0;
-        k<<<(unsigned)(n_work < slots0 ? n_work : slots0), TILE, RE_TOTAL_L0, stream>>>(a);
+        rc = pano ? launch_field<render_march_kernel<true, true, -1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, true, -1>>(RS_SMEM, WG_MAX, n_work, stream, a);
+    } else if (fast && pano && (args->flags & PERF_FLAG_L0_SMEM)) {   // experiment: level 0 in shared memory, one copy per CTA
+        rc = launch_field<render_march_kernel<true, false, 4, 0, true>>(RE_SMEM_L0, WG_MAX, n_work, stream, a);
     } else if (fast) {
-        rc = pano ? launch_field<render_march_kernel<true, false, 4>>(RE_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, 4>>(RE_LAUNCH, grid, stream, a);
+        rc = pano ? launch_field<render_march_kernel<true, false, 4>>(RE_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4>>(RE_SMEM, WG_MAX, n_work, stream, a);
     } else {
-        rc = pano ? launch_field<render_march_kernel<true, false, -1>>(RE_LAUNCH, grid, stream, a) : launch_field<render_march_kernel<false, false, -1>>(RE_LAUNCH, grid, stream, a);
+        rc = pano ? launch_field<render_march_kernel<true, false, -1>>(RE_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1>>(RE_SMEM, WG_MAX, n_work, stream, a);
     }
     if (rc) return rc;
     PERF_LAUNCH_CHECK();
@@ -1182,18 +1229,17 @@ static int fields_packed(const perf_render_args* args, const float* d_rays_o, co
     cudaStream_t st = (cudaStream_t)stream;
     rc = prepare_weights(a, st); if (rc) return rc;
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
-    const unsigned grid = (unsigned)(n_tiles < (uint64_t)num_sms() * 4 ? n_tiles : (uint64_t)num_sms() * 4);
-    // bytes: RE_TOTAL for the eval kernels (phase 0), RE_TOTAL_N for their normals twins, RS_TOTAL for the saving ones
+    // shared memory: RE_SMEM for the eval kernels (phase 0), RE_SMEM_N for their normals twins, RS_SMEM for the saving ones
     if (p.normal != nullptr) {
-        rc = fast ? launch_field<packed_fields_kernel<4, 0, true>>(RE_TOTAL_N, grid, st, a, p) : launch_field<packed_fields_kernel<-1, 0, true>>(RE_TOTAL_N, grid, st, a, p);
+        rc = fast ? launch_field<packed_fields_kernel<4, 0, true>>(RE_SMEM_N, WG_MAX, n_tiles, st, a, p) : launch_field<packed_fields_kernel<-1, 0, true>>(RE_SMEM_N, WG_MAX, n_tiles, st, a, p);
     } else if (fast) {
-        if (phase == 0) rc = launch_field<packed_fields_kernel<4, 0>>(RE_TOTAL, grid, st, a, p);
-        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<4, 1>>(RS_TOTAL, grid, st, a, p);
-        else rc = launch_field<packed_fields_kernel<4, 2>>(RS_TOTAL, grid, st, a, p);
+        if (phase == 0) rc = launch_field<packed_fields_kernel<4, 0>>(RE_SMEM, WG_MAX, n_tiles, st, a, p);
+        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<4, 1>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
+        else rc = launch_field<packed_fields_kernel<4, 2>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
     } else {
-        if (phase == 0) rc = launch_field<packed_fields_kernel<-1, 0>>(RE_TOTAL, grid, st, a, p);
-        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<-1, 1>>(RS_TOTAL, grid, st, a, p);
-        else rc = launch_field<packed_fields_kernel<-1, 2>>(RS_TOTAL, grid, st, a, p);
+        if (phase == 0) rc = launch_field<packed_fields_kernel<-1, 0>>(RE_SMEM, WG_MAX, n_tiles, st, a, p);
+        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<-1, 1>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
+        else rc = launch_field<packed_fields_kernel<-1, 2>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
     }
     if (rc) return rc;
     PERF_LAUNCH_CHECK();
@@ -1263,7 +1309,7 @@ int perf_train_forward(const perf_render_args* args, const float* d_rays_o, cons
     a.s_sigma = buf->d_sigma; a.s_w = buf->d_weights; a.s_trans = buf->d_trans; a.s_rgb = (__half*)buf->d_rgb;
     a.s_feat = (uint4*)buf->d_feat; a.s_h1 = (uint4*)buf->d_h1; a.s_h2 = (uint4*)buf->d_h2;
     a.s_dacc = buf->d_dist_acc; a.s_dl = buf->d_distloss;
-    // split rays into segments until the tiles fill the machine (4 CTAs / SM), if the caller gave room
+    // split rays into segments until the tiles fill the machine (4 tiles in flight per SM), if the caller gave room
     a.seg = 1; a.s_toff = buf->d_seg_trans;
     if (buf->d_seg_trans != nullptr) {
         const uint64_t slots = (uint64_t)num_sms() * 4;
