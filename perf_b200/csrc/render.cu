@@ -75,52 +75,6 @@ constexpr int W_IMG_BYTES = W32_BYTES + W32_BYTES + W64_BYTES;       // 16 KB: W
 constexpr int WO_BYTES = 8 * HID * 2;               // 1 KB: an output layer as an N = 8 operand image (mlp_tc.cuh layout, LBO = 128)
 constexpr int WO_LBO   = 8 * 16;
 constexpr int W_IMG_ALL = W_IMG_BYTES + 2 * WO_BYTES;                // 18 KB: the hidden images, then the two output images
-
-// Kernels that round-trip the hidden layers through shared memory: the training forward (SAVE = 1/2), the SIMT twin and
-// the legacy scan kernel.  CTA-wide block:
-constexpr int RS_W1G   = 0;
-constexpr int RS_W1A   = RS_W1G + W32_BYTES;
-constexpr int RS_W2A   = RS_W1A + W32_BYTES;
-constexpr int RS_BARW  = RS_W2A + W64_BYTES;        // mbarrier of the weight bulk copy
-constexpr int RS_CTA   = align128(RS_BARW + 16);
-// ... per warpgroup:
-constexpr int RS_A     = 0;                         // 16 KB: A_geo | A_app, later the colour hidden layers (K=64)
-constexpr int RS_H     = RS_A + A64_BYTES;          // 16 KB: density hidden layer
-constexpr int RS_TAILS = RS_H + A64_BYTES;          // [2 scans][4 warps][8] floats
-constexpr int RS_CARRY = RS_TAILS + 2 * 4 * 8 * 4;  // [2 parities][8] floats
-constexpr int RS_WG    = align128(RS_CARRY + 2 * 8 * 4);
-static_assert(RS_W1A == RS_W1G + W32_BYTES && RS_W2A == RS_W1A + W32_BYTES, "the three weight images are one contiguous block");
-static_assert(RS_CTA + WG_MAX * RS_WG + 1024 <= 164 * 1024, "4 warpgroups (+1 KB reserved) fit the 164 KB shared-memory carveout");
-
-// Eval kernels (wgmma MLP, no saves: eval_mlp_regs): the hidden layers never leave the registers, so a warpgroup needs its
-// feature tile only.  CTA-wide block:
-constexpr int RE_W1G   = 0;
-constexpr int RE_W1A   = RE_W1G + W32_BYTES;
-constexpr int RE_W2A   = RE_W1A + W32_BYTES;
-constexpr int RE_WOG   = RE_W2A + W64_BYTES;        // density output row 0, rows 1-7 zero
-constexpr int RE_WOA   = RE_WOG + WO_BYTES;         // colour output rows 0-2, rows 3-7 zero
-constexpr int RE_BARW  = RE_WOA + WO_BYTES;         // mbarrier of the weight bulk copy
-constexpr int RE_CTA   = align128(RE_BARW + 16);
-static_assert(RE_W1A == RE_W1G + W32_BYTES && RE_W2A == RE_W1A + W32_BYTES && RE_WOG == RE_W1G + W_IMG_BYTES &&
-              RE_WOA == RE_WOG + WO_BYTES, "the five weight images are one contiguous block");
-// ... per warpgroup:
-constexpr int RE_A     = 0;                         // 16 KB: A_geo | A_app
-constexpr int RE_MAX   = RE_A + A64_BYTES;          // [4 warps] longest packed ray (perf_render_packed)
-constexpr int RE_WG    = align128(RE_MAX + 16);
-static_assert(RE_CTA + WG_MAX * RE_WG + 1024 <= 100 * 1024, "4 eval warpgroups (+1 KB reserved) fit the 100 KB shared-memory carveout");
-// The normals kernels (NORMAL) append per thread the sample position and the ray's running sum w n: the layer-1 peak of
-// the MLP leaves no register for them (the eval march kernel uses all 128 without them).
-constexpr int RE_XYZ   = RE_MAX + 16;               // float4 [128]: x01, selector
-constexpr int RE_NACC  = RE_XYZ + TILE * 16;        // float [3][128]: sum w n of the thread's ray (march kernel)
-constexpr int RE_WG_N  = align128(RE_NACC + 3 * TILE * 4);
-static_assert(RE_CTA + WG_MAX * RE_WG_N + 1024 <= 100 * 1024, "4 normals warpgroups fit the 100 KB shared-memory carveout");
-// experiment (PERF_FLAG_L0_SMEM, eval layout): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in shared
-// memory behind the weights, staged once per persistent CTA by ONE bulk copy (cp.async.bulk -> UBLKCP, completion on an
-// mbarrier) and read by all its warpgroups
-constexpr int RE_BAR2  = RE_CTA;
-constexpr int RE_L0    = RE_BAR2 + 128;
-constexpr int L0_BYTES = 4096 * 8;
-constexpr int RE_CTA_L0 = RE_L0 + L0_BYTES;
 // measurement hook (tools/ab_lib.py): extra, unused dynamic shared memory per warpgroup of the field kernels, i.e. what
 // more shared memory would cost in L1 capacity
 #ifndef PERF_RS_PAD
@@ -130,17 +84,50 @@ constexpr int RE_CTA_L0 = RE_L0 + L0_BYTES;
 // Bytes the carveout percentage set_smem requests stands for on the H100 (228 KB of shared memory per SM at most): the
 // driver takes the next supported carveout at or above it, so a layout meant for a given carveout must keep this under it.
 constexpr long long carveout_request(long long need) { return (100 * need + 233471) / 233472 * 233472 / 100; }
-static_assert(carveout_request(RS_CTA + WG_MAX * RS_WG + 1024) <= 164 * 1024, "RS layout: the 164 KB carveout");
-static_assert(carveout_request(RE_CTA + WG_MAX * RE_WG + 1024) <= 100 * 1024, "eval layout: the 100 KB carveout");
-static_assert(carveout_request(RE_CTA + WG_MAX * RE_WG_N + 1024) <= 100 * 1024, "normals layout: the 100 KB carveout");
-static_assert(carveout_request(RE_CTA_L0 + WG_MAX * RE_WG + 1024) <= 132 * 1024, "level-0 layout: the 132 KB carveout");
 
-// Shared-memory shape of a field kernel: the CTA-wide block, then `nwg` regions of `wg_bytes`.
-struct FieldSmem {
-    int cta_bytes, wg_bytes;
-    int bytes(int nwg) const { return cta_bytes + nwg * (wg_bytes + PERF_RS_PAD); }
+// Shared-memory layout of a field kernel: byte offsets in the CTA-wide block, then in a warpgroup's region.
+// EVAL: the eval kernels (wgmma MLP, no saves: eval_mlp_regs) keep the hidden layers in registers, so a warpgroup needs its
+// feature tile only; the output layers are operand images too.  Otherwise the round trip: the training forward (SAVE = 1/2),
+// the SIMT twin and the legacy scan kernel pass every hidden layer through shared memory.
+// NORMAL (eval only): the normals kernels append per thread the sample position and the ray's running sum w n: the layer-1
+// peak of the MLP leaves no register for them (the eval march kernel uses all 128 without them).
+// L0SMEM (eval only, experiment PERF_FLAG_L0_SMEM): level 0 of the packed table (16^3 entries x 8 B = 32 KB) resident in
+// shared memory behind the weights, staged once per persistent CTA by ONE bulk copy and read by all its warpgroups.
+template <bool EVAL_, bool NORMAL_ = false, bool L0SMEM_ = false>
+struct FieldLayout {
+    static constexpr bool EVAL = EVAL_, NORMAL = NORMAL_, L0SMEM = L0SMEM_;
+    static_assert(EVAL || (!NORMAL && !L0SMEM), "normals and level 0 in shared memory: eval layout only");
+    // CTA-wide block: the weight operand images (W_BYTES, one bulk copy from g_wimg), the mbarrier of that copy (BARW);
+    // L0SMEM: the mbarrier of the level-0 copy and level 0
+    static constexpr int W1G = 0, W1A = W1G + W32_BYTES, W2A = W1A + W32_BYTES;
+    static constexpr int WOG = W2A + W64_BYTES, WOA = WOG + WO_BYTES;        // EVAL: density row 0 / colour rows 0-2, the rest zero
+    static constexpr int W_BYTES = EVAL ? W_IMG_ALL : W_IMG_BYTES, BARW = W1G + W_BYTES;
+    static constexpr int BARL0 = align128(BARW + 16), L0 = BARL0 + 128, L0_BYTES = 4096 * 8;
+    static constexpr int CTA = L0SMEM ? L0 + L0_BYTES : align128(BARW + 16);
+    static_assert(W1A == W1G + W32_BYTES && W2A == W1A + W32_BYTES && WOG == W1G + W_IMG_BYTES && WOA == WOG + WO_BYTES,
+                  "the weight images are one contiguous block, the layout of g_wimg");
+    // per warpgroup: A = A_geo | A_app (16 KB; in the round trip later the colour hidden layers, K = 64); round trip: H = the
+    // density hidden layer (16 KB), render_kernel's scan TAILS [2 scans][4 warps][8] and CARRY [2 parities][8] floats
+    static constexpr int A = 0, H = A + A64_BYTES, TAILS = H + A64_BYTES, CARRY = TAILS + 2 * 4 * 8 * 4;
+    // [4 warps] longest packed ray (perf_render_packed); the round trip aliases the tails: the scan kernel renders no packed rays
+    static constexpr int MAX = EVAL ? A + A64_BYTES : TAILS;
+    static constexpr int XYZ = MAX + 16, NACC = XYZ + TILE * 16;             // NORMAL: float4 [128] x01, selector; float [3][128] sum w n
+    static constexpr int WG = align128(!EVAL ? CARRY + 2 * 8 * 4 : NORMAL ? NACC + 3 * TILE * 4 : MAX + 16);
+    static constexpr int bytes(int nwg) { return CTA + nwg * (WG + PERF_RS_PAD); }   // the CTA-wide block, then nwg regions
 };
-constexpr FieldSmem RS_SMEM = {RS_CTA, RS_WG}, RE_SMEM = {RE_CTA, RE_WG}, RE_SMEM_N = {RE_CTA, RE_WG_N}, RE_SMEM_L0 = {RE_CTA_L0, RE_WG};
+// WG_MAX warpgroups of layout L take `total` bytes (PERF_RS_PAD aside), and with the 1 KB reserved per CTA they fit the
+// `kb` KB carveout.  The four layouts, as DESIGN.md section 3 quotes them:
+template <class L> constexpr bool layout_is(int total, int kb) { return L::CTA + WG_MAX * L::WG == total && carveout_request(total + 1024) <= kb * 1024; }
+static_assert(layout_is<FieldLayout<true>>(18560 + 4 * 16512, 100), "eval layout: 84 608 B, the 100 KB carveout");
+static_assert(layout_is<FieldLayout<true, true>>(18560 + 4 * 20096, 100), "normals layout: 98 944 B, the 100 KB carveout");
+static_assert(layout_is<FieldLayout<false>>(16512 + 4 * 33152, 164), "round-trip layout: 149 120 B, the 164 KB carveout");
+static_assert(layout_is<FieldLayout<true, false, true>>(117504, 132), "level-0 layout: 117 504 B, the 132 KB carveout");
+// The layout of each field kernel, read by the kernel and by its launch (launch_march, launch_packed, launch_scan).
+// render_march_kernel<PANO, SIMT, NDENSE, SAVE, L0SMEM, NORMAL> and packed_fields_kernel<NDENSE, SAVE, NORMAL> (SIMT = false):
+// the eval layout unless the MLP runs on CUDA cores or saves.  render_kernel: the round trip.
+template <bool SIMT, int SAVE, bool L0SMEM = false, bool NORMAL = false>
+using MarchLayout = FieldLayout<!SIMT && SAVE == 0, NORMAL, L0SMEM>;
+using ScanLayout = FieldLayout<false>;
 
 // Output-layer weights of both networks as fp32 in the CONSTANT bank: [0,64) density row, [64,256) the three colour
 // rows.  The 64 * n_out FMAs per sample of the output layers then take their weight operand straight from c[bank][imm]
@@ -172,18 +159,17 @@ __global__ void __launch_bounds__(1024) weights_prepare_kernel(const __half* __r
     }
 }
 
-// all threads of the CTA: weight images global -> the CTA-wide block of shared memory by one bulk copy; returns when they
-// have landed.  EVAL: the eval layout (RE_*, all five images); otherwise RS_* and the three hidden-layer images.
-template <bool EVAL>
+// all threads of the CTA: weight images global -> the CTA-wide block of layout L by one bulk copy; returns when they have
+// landed.  The eval layout takes all five images, the round trip the three hidden-layer ones.
+template <class L>
 __device__ __forceinline__ void stage_weights_bulk(uint8_t* smem)
 {
-    constexpr int bytes = EVAL ? W_IMG_ALL : W_IMG_BYTES;
-    uint64_t* barw = reinterpret_cast<uint64_t*>(smem + (EVAL ? RE_BARW : RS_BARW));
+    uint64_t* barw = reinterpret_cast<uint64_t*>(smem + L::BARW);
     if (threadIdx.x == 0) {
         mbar_init(barw, 1); fence_mbar_init();
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(barw)), "r"(bytes) : "memory");
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(barw)), "r"(L::W_BYTES) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     :: "r"(smem_u32(smem + (EVAL ? RE_W1G : RS_W1G))), "l"(reinterpret_cast<const void*>(g_wimg)), "r"(bytes), "r"(smem_u32(barw)) : "memory");
+                     :: "r"(smem_u32(smem + L::W1G)), "l"(reinterpret_cast<const void*>(g_wimg)), "r"(L::W_BYTES), "r"(smem_u32(barw)) : "memory");
     }
     __syncthreads();                                 // the barrier is initialised before anyone polls it
     mbar_wait(barw, 0);
@@ -294,6 +280,19 @@ struct RenderSmem {
     const uint2* l0;        // level 0 of the packed table in shared memory, or null
     float4* xyz;            // NORMAL kernels: [128] each thread's sample position + selector across the MLP, or null
 };
+
+// Warpgroup wg's view of a field kernel's shared memory in layout L (wg warp-uniform: see render_march_kernel): the
+// RenderSmem, and the start of the warpgroup's region in `region` (not a member of RenderSmem: one there changes the SASS).
+template <class L>
+__device__ __forceinline__ RenderSmem field_smem(uint8_t* smem, int wg, uint8_t*& region)
+{
+    region = smem + (L::CTA + wg * L::WG) + wg * PERF_RS_PAD;
+    uint8_t* const sA = region + L::A;
+    return {sA, sA, sA + A32_BYTES, L::EVAL ? nullptr : region + L::H, smem + L::W1G, smem + L::W1A, smem + L::W2A,
+            L::EVAL ? smem + L::WOG : nullptr, L::EVAL ? smem + L::WOA : nullptr,
+            L::L0SMEM ? reinterpret_cast<const uint2*>(smem + L::L0) : nullptr,
+            L::NORMAL ? reinterpret_cast<float4*>(region + L::XYZ) : nullptr};
+}
 
 // base + 8 * idx as ONE IMAD.WIDE.U32 (left to itself ptxas splits the 64-bit address into LEA + IADD3.X per corner)
 __device__ __forceinline__ const uint2* entry_ptr(const uint2* base, uint32_t idx)
@@ -681,22 +680,14 @@ __device__ __forceinline__ void eval_fields(const RenderArgs& a, const RenderSme
 template <bool PANO, bool SIMT>
 __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__ RenderArgs a)
 {
+    using L = ScanLayout;                            // one warpgroup per CTA (launch_scan)
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* const wgs = smem + RS_CTA;     // the one warpgroup's region
-    uint8_t* sA   = wgs + RS_A;
-    uint8_t* sAg  = sA;                     // geo features, K=32
-    uint8_t* sAa  = sA + A32_BYTES;         // app features, K=32
-    uint8_t* sH   = wgs + RS_H;
-    uint8_t* sW1g = smem + RS_W1G;
-    uint8_t* sW1a = smem + RS_W1A;
-    uint8_t* sW2a = smem + RS_W2A;
-    float*   sTails = reinterpret_cast<float*>(wgs + RS_TAILS);
-    float*   sCarry = reinterpret_cast<float*>(wgs + RS_CARRY);
-
+    uint8_t* wgs; const RenderSmem sm = field_smem<L>(smem, 0, wgs);
+    float* const sTails = reinterpret_cast<float*>(wgs + L::TAILS);
+    float* const sCarry = reinterpret_cast<float*>(wgs + L::CARRY);
     const int tid = threadIdx.x;
-    const RenderSmem sm = {sA, sAg, sAa, sH, sW1g, sW1a, sW2a, nullptr, nullptr, nullptr};
 
-    stage_weights_bulk<false>(smem);                 // W1 density | W1 colour | W2 colour operand images, one bulk copy
+    stage_weights_bulk<L>(smem);                     // W1 density | W1 colour | W2 colour operand images, one bulk copy
 
     const uint32_t S = a.S;
     const float step = fixed_s_step(a.near, a.far, S);
@@ -794,30 +785,22 @@ __global__ void __launch_bounds__(TILE, 4) render_kernel(const __grid_constant__
 template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false, bool NORMAL = false>
 __global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __grid_constant__ RenderArgs a)
 {
-    constexpr bool EVAL = !SIMT && SAVE == 0;        // hidden layers in registers, eval shared-memory layout (RE_*)
+    using L = MarchLayout<SIMT, SAVE, L0SMEM, NORMAL>;   // L::EVAL: hidden layers in registers, eval shared-memory layout
     extern __shared__ __align__(128) uint8_t smem[];
     // wg broadcast from lane 0: the compiler then knows it is warp-uniform and keeps the region's address and the wgmma
     // descriptors built from it in uniform registers (threadIdx.x / TILE alone costs the 128-register kernels spills)
     const int wg = __shfl_sync(0xffffffffu, threadIdx.x / TILE, 0), nwg = blockDim.x / TILE;
-    uint8_t* const wgs = smem + (EVAL ? (L0SMEM ? RE_CTA_L0 : RE_CTA) + wg * (NORMAL ? RE_WG_N : RE_WG) : RS_CTA + wg * RS_WG) +
-                         wg * PERF_RS_PAD;       // this warpgroup's region
-    uint8_t* sA   = wgs + (EVAL ? RE_A : RS_A);
-
+    uint8_t* wgs; const RenderSmem sm = field_smem<L>(smem, wg, wgs);
     const int tid = NORMAL ? (int)(threadIdx.x % TILE) : (int)threadIdx.x - wg * TILE, warp = tid >> 5, lane = tid & 31;
-    const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
-                                            smem + RE_WOA, L0SMEM ? reinterpret_cast<const uint2*>(smem + RE_L0) : nullptr,
-                                            NORMAL ? reinterpret_cast<float4*>(wgs + RE_XYZ) : nullptr}
-                               : RenderSmem{sA, sA, sA + A32_BYTES, wgs + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
-                                            nullptr, nullptr};
 
-    stage_weights_bulk<EVAL>(smem);                  // the weight operand images, one bulk copy
+    stage_weights_bulk<L>(smem);                     // the weight operand images, one bulk copy
     if constexpr (L0SMEM) {
-        uint64_t* bar2 = reinterpret_cast<uint64_t*>(smem + RE_BAR2);
+        uint64_t* bar2 = reinterpret_cast<uint64_t*>(smem + L::BARL0);
         if (threadIdx.x == 0) {
             mbar_init(bar2, 1); fence_mbar_init();
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar2)), "r"(L0_BYTES) : "memory");
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar2)), "r"(L::L0_BYTES) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"(smem_u32(smem + RE_L0)), "l"(a.table), "r"(L0_BYTES), "r"(smem_u32(bar2)) : "memory");
+                         :: "r"(smem_u32(smem + L::L0)), "l"(a.table), "r"(L::L0_BYTES), "r"(smem_u32(bar2)) : "memory");
         }
         __syncthreads();                                   // the barrier is initialised before anyone polls it
         mbar_wait(bar2, 0);
@@ -888,7 +871,7 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __
         float sum_sd = 0.f;                                   // exclusive running sum of sigma*dt
         float acc_w = 0.f, acc_d = 0.f, acc_r = 0.f, acc_g = 0.f, acc_b = 0.f;
         float dl_uni = 0.f, dl_bi = 0.f;                      // distortion loss pieces (SAVE only)
-        float* const acc_n = reinterpret_cast<float*>(wgs + RE_NACC) + tid;        // sum w n (NORMAL only): [3][128]
+        float* const acc_n = reinterpret_cast<float*>(wgs + L::NACC) + tid;  // sum w n (NORMAL only): [3][128]
         if constexpr (NORMAL) { acc_n[0] = 0.f; acc_n[TILE] = 0.f; acc_n[2 * TILE] = 0.f; }
         // packed mode: every thread walks ITS ray's samples; the tile iterates to the longest ray
         // (neighbouring rays cross the same occupied shells, so lengths inside a tile are similar)
@@ -898,7 +881,7 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __
             my_count = 0;
             if (valid) { pk_base = a.pk_offsets[ray]; my_count = (uint32_t)(a.pk_offsets[ray + 1] - pk_base); }
             const uint32_t wmax = __reduce_max_sync(0xffffffffu, my_count);
-            uint32_t* s_max = reinterpret_cast<uint32_t*>(wgs + (EVAL ? RE_MAX : RS_TAILS));
+            uint32_t* s_max = reinterpret_cast<uint32_t*>(wgs + L::MAX);
             wg_sync();                                        // previous tile's readers are done
             if (lane == 0) s_max[warp] = wmax;
             wg_sync();
@@ -923,7 +906,7 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __
 
             float sigma, cr, cg, cb, nrm[3];
             const uint64_t srow = (SAVE != 0 && valid) ? (uint64_t)k * a.R + ray : ~0ull;
-            eval_fields<SIMT, NDENSE, SAVE, EVAL, L0SMEM, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow, nrm);
+            eval_fields<SIMT, NDENSE, SAVE, L::EVAL, L0SMEM, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, srow, nrm);
 
             const float dt = __fsub_rn(te, ts);
             const float sd = sigma * dt;
@@ -957,7 +940,7 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) render_march_kernel(const __
         if (seg > 1) {
             // combine the `seg` partial composites of every ray (each computed as if T = 1 at the segment
             // start): w = Toff w', Wx = Wpre + Toff Wx', ... ; scratch = the (now idle) feature tiles
-            float* part = reinterpret_cast<float*>(sA);
+            float* part = reinterpret_cast<float*>(sm.sA);
             wg_sync();
             part[0 * TILE + tid] = sum_sd; part[1 * TILE + tid] = acc_w; part[2 * TILE + tid] = acc_d;
             part[3 * TILE + tid] = acc_r;  part[4 * TILE + tid] = acc_g; part[5 * TILE + tid] = acc_b;
@@ -1025,17 +1008,12 @@ struct PackedFieldArgs {
 template <int NDENSE, int SAVE, bool NORMAL = false>
 __global__ void __launch_bounds__(WG_MAX * TILE, 1) packed_fields_kernel(const __grid_constant__ RenderArgs a, const PackedFieldArgs p)
 {
-    constexpr bool EVAL = SAVE == 0;                 // hidden layers in registers, eval shared-memory layout (RE_*)
+    using L = MarchLayout<false, SAVE, false, NORMAL>;   // L::EVAL: hidden layers in registers, eval shared-memory layout
     extern __shared__ __align__(128) uint8_t smem[];
     const int wg = __shfl_sync(0xffffffffu, threadIdx.x / TILE, 0), nwg = blockDim.x / TILE;   // warp-uniform: see render_march_kernel
-    uint8_t* const wgs = smem + (EVAL ? RE_CTA + wg * (NORMAL ? RE_WG_N : RE_WG) : RS_CTA + wg * RS_WG) + wg * PERF_RS_PAD;
-    uint8_t* sA   = wgs + (EVAL ? RE_A : RS_A);
+    uint8_t* wgs; const RenderSmem sm = field_smem<L>(smem, wg, wgs);
     const int tid = threadIdx.x % TILE;
-    const RenderSmem sm = EVAL ? RenderSmem{sA, sA, sA + A32_BYTES, nullptr, smem + RE_W1G, smem + RE_W1A, smem + RE_W2A, smem + RE_WOG,
-                                            smem + RE_WOA, nullptr, NORMAL ? reinterpret_cast<float4*>(wgs + RE_XYZ) : nullptr}
-                               : RenderSmem{sA, sA, sA + A32_BYTES, wgs + RS_H, smem + RS_W1G, smem + RS_W1A, smem + RS_W2A, nullptr,
-                                            nullptr, nullptr};
-    stage_weights_bulk<EVAL>(smem);                  // the weight operand images, one bulk copy
+    stage_weights_bulk<L>(smem);                     // the weight operand images, one bulk copy
     uint64_t N = p.N;
     if (p.n_dev) { const int64_t nd = *p.n_dev; N = nd < 0 ? 0 : ((uint64_t)nd < N ? (uint64_t)nd : N); }      // graph-replayable count
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
@@ -1056,7 +1034,7 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) packed_fields_kernel(const _
         }
         const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
         float sigma, cr, cg, cb, nrm[3];
-        eval_fields<false, NDENSE, SAVE, EVAL, false, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull, nrm);
+        eval_fields<false, NDENSE, SAVE, L::EVAL, false, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, valid ? n : ~0ull, nrm);
         if (valid) {
             p.sigma[n] = sigma;
             if constexpr (NORMAL) { p.normal[3 * n] = nrm[0]; p.normal[3 * n + 1] = nrm[1]; p.normal[3 * n + 2] = nrm[2]; }
@@ -1099,22 +1077,23 @@ static int set_smem(K k, int bytes, int ctas)
     return PERF_OK;
 }
 
-// Launch of field kernel K over n_work 128-row tiles, WG_MAX tiles in flight per SM.  nwg_max = WG_MAX (render_march_kernel,
-// packed_fields_kernel): one CTA per SM of nwg = clamp(ceil(n_work / SMs), 1, WG_MAX) warpgroups that share one copy of the
-// weights, so a small launch still spreads one tile per SM.  nwg_max = 1 (the legacy scan kernel): WG_MAX 128-thread CTAs
-// per SM.  Once per device and kernel: the carveout for the nwg_max shape (set_smem), and a check that it is resident.
-template <auto K, class... P>
-static int launch_field(const FieldSmem& fs, int nwg_max, uint64_t n_work, cudaStream_t stream, const P&... p)
+// Launch of field kernel K, whose shared memory is layout L, over n_work 128-row tiles, WG_MAX tiles in flight per SM.
+// nwg_max = WG_MAX (render_march_kernel, packed_fields_kernel): one CTA per SM of nwg = clamp(ceil(n_work / SMs), 1, WG_MAX)
+// warpgroups that share one copy of the weights, so a small launch still spreads one tile per SM.  nwg_max = 1 (the legacy
+// scan kernel): WG_MAX 128-thread CTAs per SM.  Once per device and kernel: the carveout for the nwg_max shape (set_smem),
+// and a check that it is resident.  Called by launch_march, launch_packed and launch_scan only, which pick K and L together.
+template <auto K, class L, class... P>
+static int launch_field(int nwg_max, uint64_t n_work, cudaStream_t stream, const P&... p)
 {
     static thread_local int attr_dev = -1;
     const int ctas_per_sm = WG_MAX / nwg_max;
     int dev = 0; PERF_CUDA(cudaGetDevice(&dev));
     if (attr_dev != dev) {
-        const int rc = set_smem(K, fs.bytes(nwg_max), ctas_per_sm); if (rc) return rc;
+        const int rc = set_smem(K, L::bytes(nwg_max), ctas_per_sm); if (rc) return rc;
         int resident = 0;
-        PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, K, nwg_max * TILE, fs.bytes(nwg_max)));
+        PERF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, K, nwg_max * TILE, L::bytes(nwg_max)));
         PERF_CHECK_SUP(resident >= ctas_per_sm, "field kernel: %d CTAs of %d threads and %d B of shared memory per SM, %d resident",
-                       ctas_per_sm, nwg_max * TILE, fs.bytes(nwg_max), resident);
+                       ctas_per_sm, nwg_max * TILE, L::bytes(nwg_max), resident);
         attr_dev = dev;
     }
     const uint64_t ctas = (uint64_t)num_sms() * ctas_per_sm;
@@ -1122,8 +1101,26 @@ static int launch_field(const FieldSmem& fs, int nwg_max, uint64_t n_work, cudaS
     const int nwg = want < (uint64_t)nwg_max ? (int)want : nwg_max;
     const uint64_t need = (n_work + nwg - 1) / nwg;
     const unsigned grid = (unsigned)(need < ctas ? need : ctas);
-    K<<<grid, nwg * TILE, fs.bytes(nwg), stream>>>(p...);
+    K<<<grid, nwg * TILE, L::bytes(nwg), stream>>>(p...);
     return PERF_OK;
+}
+
+template <bool PANO, bool SIMT, int NDENSE, int SAVE = 0, bool L0SMEM = false, bool NORMAL = false>
+static int launch_march(uint64_t n_work, cudaStream_t stream, const RenderArgs& a)
+{
+    return launch_field<render_march_kernel<PANO, SIMT, NDENSE, SAVE, L0SMEM, NORMAL>, MarchLayout<SIMT, SAVE, L0SMEM, NORMAL>>(WG_MAX, n_work, stream, a);
+}
+
+template <bool PANO, bool SIMT>
+static int launch_scan(uint64_t n_work, cudaStream_t stream, const RenderArgs& a)
+{
+    return launch_field<render_kernel<PANO, SIMT>, ScanLayout>(1, n_work, stream, a);
+}
+
+template <int NDENSE, int SAVE, bool NORMAL = false>
+static int launch_packed(uint64_t n_work, cudaStream_t stream, const RenderArgs& a, const PackedFieldArgs& p)
+{
+    return launch_field<packed_fields_kernel<NDENSE, SAVE, NORMAL>, MarchLayout<false, SAVE, false, NORMAL>>(WG_MAX, n_work, stream, a, p);
 }
 
 // The part of RenderArgs every field kernel needs: level table, packed table and its cell-major copies, weights, aabb and
@@ -1146,6 +1143,23 @@ static int init_field_args(const perf_render_args* args, RenderArgs& a, bool& fa
     for (int i = 0; i < 3; ++i) if (!div_uniform_ok(a.aabb_ext[i])) a.div_generic = 1u;
     fast = fast_addressing_ok(a.lt, 4) && pl.n_cell_levels == 4 && (args->flags & PERF_FLAG_GENERIC_ADDR) == 0;
     return PERF_OK;
+}
+
+// The render kernel for PANO and NDENSE (4: fast addressing, -1: generic), in launch_render's order of precedence; a
+// training forward (save != 0) is neither a panorama nor SIMT nor scan (launch_render refuses those).
+template <bool PANO, int NDENSE>
+static int render_kernels(uint64_t n_work, cudaStream_t stream, const RenderArgs& a, int save, bool normals, bool simt, bool scan, bool l0)
+{
+    if (normals) return launch_march<PANO, false, NDENSE, 0, false, true>(n_work, stream, a);   // eval march kernel only (the callers refuse the rest)
+    if constexpr (!PANO) {
+        if (save != 0) return save == 1 ? launch_march<false, false, NDENSE, 1>(n_work, stream, a) : launch_march<false, false, NDENSE, 2>(n_work, stream, a);
+    }
+    if (scan) return simt ? launch_scan<PANO, true>(n_work, stream, a) : launch_scan<PANO, false>(n_work, stream, a);   // legacy scan kernel
+    if (simt) return launch_march<PANO, true, -1>(n_work, stream, a);
+    if constexpr (PANO && NDENSE == 4) {
+        if (l0) return launch_march<true, false, 4, 0, true>(n_work, stream, a);   // experiment: level 0 in shared memory, one copy per CTA
+    }
+    return launch_march<PANO, false, NDENSE>(n_work, stream, a);
 }
 
 // normals: a.normal is set (it shares its slot with a.s_toff, so only this flag selects the NORMAL kernels)
@@ -1185,26 +1199,10 @@ static int launch_render(const perf_render_args* args, RenderArgs& a, bool pano,
         a.tile_mul = m % (uint32_t)n_work;
     }
     rc = prepare_weights(a, stream); if (rc) return rc;     // constant-bank output weights + operand images (c_wout, g_wimg)
-    // shared memory: RE_SMEM for the eval kernels (SIMT = false, SAVE = 0), RE_SMEM_N for their normals twins, RS_SMEM for the others
-    if (normals) {                                                // surface normals: eval march kernel only (the callers refuse the rest)
-        if (fast) rc = pano ? launch_field<render_march_kernel<true, false, 4, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a);
-        else      rc = pano ? launch_field<render_march_kernel<true, false, -1, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1, 0, false, true>>(RE_SMEM_N, WG_MAX, n_work, stream, a);
-    } else if (save != 0) {
-        PERF_CHECK_SUP(!pano && !simt && !scan, "training forward runs on the ray-marching tensor-core kernel only");
-        if (fast) rc = save == 1 ? launch_field<render_march_kernel<false, false, 4, 1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4, 2>>(RS_SMEM, WG_MAX, n_work, stream, a);
-        else      rc = save == 1 ? launch_field<render_march_kernel<false, false, -1, 1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1, 2>>(RS_SMEM, WG_MAX, n_work, stream, a);
-    } else if (scan) {                                            // legacy scan kernel: 128-thread CTAs
-        if (pano) rc = simt ? launch_field<render_kernel<true, true>>(RS_SMEM, 1, n_work, stream, a) : launch_field<render_kernel<true, false>>(RS_SMEM, 1, n_work, stream, a);
-        else      rc = simt ? launch_field<render_kernel<false, true>>(RS_SMEM, 1, n_work, stream, a) : launch_field<render_kernel<false, false>>(RS_SMEM, 1, n_work, stream, a);
-    } else if (simt) {
-        rc = pano ? launch_field<render_march_kernel<true, true, -1>>(RS_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, true, -1>>(RS_SMEM, WG_MAX, n_work, stream, a);
-    } else if (fast && pano && (args->flags & PERF_FLAG_L0_SMEM)) {   // experiment: level 0 in shared memory, one copy per CTA
-        rc = launch_field<render_march_kernel<true, false, 4, 0, true>>(RE_SMEM_L0, WG_MAX, n_work, stream, a);
-    } else if (fast) {
-        rc = pano ? launch_field<render_march_kernel<true, false, 4>>(RE_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, 4>>(RE_SMEM, WG_MAX, n_work, stream, a);
-    } else {
-        rc = pano ? launch_field<render_march_kernel<true, false, -1>>(RE_SMEM, WG_MAX, n_work, stream, a) : launch_field<render_march_kernel<false, false, -1>>(RE_SMEM, WG_MAX, n_work, stream, a);
-    }
+    PERF_CHECK_SUP(save == 0 || (!pano && !simt && !scan), "training forward runs on the ray-marching tensor-core kernel only");
+    const bool l0 = (args->flags & PERF_FLAG_L0_SMEM) != 0;
+    if (pano) rc = fast ? render_kernels<true, 4>(n_work, stream, a, save, normals, simt, scan, l0) : render_kernels<true, -1>(n_work, stream, a, save, normals, simt, scan, l0);
+    else      rc = fast ? render_kernels<false, 4>(n_work, stream, a, save, normals, simt, scan, l0) : render_kernels<false, -1>(n_work, stream, a, save, normals, simt, scan, l0);
     if (rc) return rc;
     PERF_LAUNCH_CHECK();
     return PERF_OK;
@@ -1229,18 +1227,10 @@ static int fields_packed(const perf_render_args* args, const float* d_rays_o, co
     cudaStream_t st = (cudaStream_t)stream;
     rc = prepare_weights(a, st); if (rc) return rc;
     const uint64_t n_tiles = (N + TILE - 1) / TILE;
-    // shared memory: RE_SMEM for the eval kernels (phase 0), RE_SMEM_N for their normals twins, RS_SMEM for the saving ones
-    if (p.normal != nullptr) {
-        rc = fast ? launch_field<packed_fields_kernel<4, 0, true>>(RE_SMEM_N, WG_MAX, n_tiles, st, a, p) : launch_field<packed_fields_kernel<-1, 0, true>>(RE_SMEM_N, WG_MAX, n_tiles, st, a, p);
-    } else if (fast) {
-        if (phase == 0) rc = launch_field<packed_fields_kernel<4, 0>>(RE_SMEM, WG_MAX, n_tiles, st, a, p);
-        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<4, 1>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
-        else rc = launch_field<packed_fields_kernel<4, 2>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
-    } else {
-        if (phase == 0) rc = launch_field<packed_fields_kernel<-1, 0>>(RE_SMEM, WG_MAX, n_tiles, st, a, p);
-        else if (phase == PERF_PHASE_GEO) rc = launch_field<packed_fields_kernel<-1, 1>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
-        else rc = launch_field<packed_fields_kernel<-1, 2>>(RS_SMEM, WG_MAX, n_tiles, st, a, p);
-    }
+    if (p.normal != nullptr) rc = fast ? launch_packed<4, 0, true>(n_tiles, st, a, p) : launch_packed<-1, 0, true>(n_tiles, st, a, p);
+    else if (phase == 0) rc = fast ? launch_packed<4, 0>(n_tiles, st, a, p) : launch_packed<-1, 0>(n_tiles, st, a, p);
+    else if (phase == PERF_PHASE_GEO) rc = fast ? launch_packed<4, 1>(n_tiles, st, a, p) : launch_packed<-1, 1>(n_tiles, st, a, p);
+    else rc = fast ? launch_packed<4, 2>(n_tiles, st, a, p) : launch_packed<-1, 2>(n_tiles, st, a, p);
     if (rc) return rc;
     PERF_LAUNCH_CHECK();
     return PERF_OK;
