@@ -362,6 +362,56 @@ int perf_hashgrid_bwd_merged(const perf_grid_cfg* cfg, const float* d_x01, const
  * graph and replayed without a host read.  perf_occ_write's `capacity` (0 = unlimited) drops samples that would not fit; the
  * caller clamps the offsets and the count to it. */
 
+/* ---- normal-consistency loss of the density phase (MonoSDF's L1 + angular normal loss against the supervision normals that
+ * SupInfoPool.rand_ray_color_data returns, sup_info.py:236-259, and train_one_step_geo drops, nerf.py:193).  Definition, per sample i
+ * of a density-phase training step at normalised position x01:
+ *   h1 = the fp16 layer-1 activation the training forward saved, m = [h1 > 0] (the eval normals' m = [h > 0] on the fp32 h differs
+ *   only where 0 < h < 2^-25, which rounds to an fp16 zero), g = W1^T (m . w_out) (fp16 shadow weights as fp32),
+ *   grad01 = sum_levels of perf_hashgrid_bwd_input's arithmetic with dL/dfeature = g on the fp16 geo table, grad = grad01 / aabb extent,
+ *   n_i = -grad / |grad|, and n_i = 0 when the selector is false, |grad| = 0, w_i = 0 or T_i = 0 (a dropped sample).
+ * Ray normal N_r = sum_i sg(w_i) n_i (the weights are detached: the loss turns the density gradient where the surface already is).
+ * Loss: g^_r = gt_r / |gt_r|; ray r is valid iff |gt_r| > 0.5 and |N_r| > 1e-6; N^_r = N_r / |N_r|;
+ *   l_r = |N^_r - g^_r|_1 + (1 - N^_r . g^_r),  L_n = sum_valid l_r / max(#valid, 1),
+ *   dl/dN = (I - N^ N^T)(sign(N^ - g^) - g^) / |N| with sign(0) = 0.
+ * The supervision normals point toward the camera (the orientation of -grad raw); pools without a normal map hold zeros. */
+typedef struct perf_sample_layout {
+    uint64_t R;                    /* rays                                                                                   */
+    uint64_t N;                    /* sample rows: R * n_samples (fixed-S) or the capacity of the packed buffers             */
+    float    aabb[6];              /* the renderer's box (min xyz, max xyz)                                                  */
+    /* packed (occupancy) layout, selected by d_x01 != NULL: samples sorted by ray, as perf_fields_packed saved them          */
+    const float*   d_x01;          /* [N,3] perf_fields_packed's saved normalised positions                                   */
+    const int64_t* d_offsets;      /* [R+1] per-ray ranges                                                                    */
+    const int64_t* d_ray_indices;  /* [N] (perf_normals_train_bwd only)                                                       */
+    const int64_t* d_n_dev;        /* nullable: live sample count in device memory (<= N), as perf_fields_packed             */
+    /* fixed-S layout (d_x01 == NULL): sample-major rows k * R + ray, positions recomputed from the rays bit for bit as the forward */
+    const float* d_rays_o;         /* [R,3]                                                                                   */
+    const float* d_rays_d;         /* [R,3]                                                                                   */
+    const float* d_jitter;         /* [R] or NULL                                                                             */
+    uint32_t n_samples, segments;  /* S and the segment count perf_train_forward chose (perf_train_buffers)                   */
+    float near, far;
+    const float* d_seg_trans;      /* perf_train_buffers::d_seg_trans when segments > 1                                       */
+} perf_sample_layout;
+/* Sample normals and ray normals of a density-phase step.  d_params_half: the density net's fp16 flat params (MLP | grid; 16 levels,
+ * 32 -> 64 -> 1, else PERF_EUNSUPPORTED); d_h1 [N,64] fp16, d_weights / d_trans [N]: the step's saves (perf_train_forward /
+ * perf_fields_packed + perf_composite_packed_fwd).  Writes d_sample_normal [N,3] = n_i, d_inv_norm [N] = 1 / |grad| (0 where n_i = 0)
+ * and d_ray_normal [R,3] = N_r (deterministic: a fixed summation order per ray, no atomics). */
+int perf_normals_train_fwd(const perf_grid_cfg* grid, const perf_mlp_cfg* mlp, const void* d_params_half, const perf_sample_layout* layout,
+                           const void* d_h1, const float* d_weights, const float* d_trans,
+                           float* d_sample_normal, float* d_inv_norm, float* d_ray_normal, void* stream);
+/* The loss above in one launch: d_loss2 = {L_n, #valid}; d_g_ray_normal [R,3] = dL_n / dN_r (unscaled, 0 on invalid rays).
+ * d_ray_normal / d_gt_normal [R,3].  The valid count stays on the device. */
+int perf_normal_loss(const float* d_ray_normal, const float* d_gt_normal, uint64_t R, float* d_loss2, float* d_g_ray_normal, void* stream);
+/* Backward of the ray normals into the density net: with G_r = d_g_ray_normal [R,3] and u = -(I - n n^T)(w_i G_r) / |grad|,
+ * v = u / aabb extent (= dL/d grad01), per level dg = sum_d v_d scale s' A_d (the dfeat branch of perf_hashgrid_bwd_bwd_input) and the
+ * table term of the same function; P = sum_i m_i (x) dg_i (64 x 32), dW1 = diag(w_out) P, dw_out_j = sum_k W1_jk P_jk.
+ * d_sample_normal / d_inv_norm: perf_normals_train_fwd's outputs.  d_dparams [n_mlp + 2 n_entries] fp32 in the flat parameter layout
+ * (MLP | grid), ACCUMULATED (fp32 atomics; the caller zeroes it, or passes the step's gradient).  Samples with w_i |G_r| = 0 issue
+ * nothing. */
+int perf_normals_train_bwd(const perf_grid_cfg* grid, const perf_mlp_cfg* mlp, const void* d_params_half, const perf_sample_layout* layout,
+                           const void* d_h1, const float* d_weights, const float* d_trans,
+                           const float* d_sample_normal, const float* d_inv_norm, const float* d_g_ray_normal,
+                           float* d_dparams, void* stream);
+
 /* Batch draw (sup_info.py:253-259): dst_k[b, :] = src_k[idx[b], :] for up to 6 row-major fp32 arrays of row widths
  * h_width[k] in one launch.  h_src / h_dst: HOST arrays of device pointers. */
 int perf_gather_rows(const int64_t* d_idx, uint64_t B, int n_arrays, const float* const* h_src, float* const* h_dst, const int* h_width, void* stream);

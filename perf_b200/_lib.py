@@ -48,6 +48,12 @@ class TrainBuffers(C.Structure):
                 ("d_h2", vp), ("d_dist_acc", vp), ("d_distloss", vp), ("d_seg_trans", vp), ("h_segments_out", P_u32)]
 
 
+class SampleLayout(C.Structure):
+    _fields_ = [("R", u64), ("N", u64), ("aabb", f32 * 6), ("d_x01", vp), ("d_offsets", vp), ("d_ray_indices", vp), ("d_n_dev", vp),
+                ("d_rays_o", vp), ("d_rays_d", vp), ("d_jitter", vp), ("n_samples", u32), ("segments", u32), ("near", f32), ("far", f32),
+                ("d_seg_trans", vp)]
+
+
 PERF_PHASE_GEO, PERF_PHASE_APP = 1, 2
 
 P = C.POINTER
@@ -90,6 +96,9 @@ SIGNATURES = {
     "perf_composite_packed_fwd": (i32, [vp, vp, vp, vp, vp, u64, f32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_composite_packed_bwd": (i32, [i32, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_hashgrid_bwd_merged": (i32, [P(GridCfg), vp, vp, u64, vp, vp, u32, vp]),
+    "perf_normals_train_fwd": (i32, [P(GridCfg), P(MlpCfg), vp, P(SampleLayout), vp, vp, vp, vp, vp, vp, vp]),
+    "perf_normal_loss": (i32, [vp, vp, u64, vp, vp, vp]),
+    "perf_normals_train_bwd": (i32, [P(GridCfg), P(MlpCfg), vp, P(SampleLayout), vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_gather_rows": (i32, [vp, u64, i32, vp, vp, vp, vp]),
     "perf_draw_gather_rows": (i32, [vp, u64, u64, vp, i32, vp, vp, vp, vp]),
     "perf_train_loss": (i32, [vp, vp, u64, u64, f32, f32, vp, vp, vp, f32, vp, vp, vp, vp]),

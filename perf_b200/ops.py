@@ -738,7 +738,7 @@ class _FusedTrainStep(torch.autograd.Function):
     (perf_train_forward), backward = composite-backward kernel, ONE wgmma MLP-backward kernel, grid scatter."""
 
     @staticmethod
-    def forward(ctx, params, rays_o, rays_d, jitter, bg_noise, tc: FusedTrainContext, phase: int):
+    def forward(ctx, params, rays_o, rays_d, jitter, bg_noise, tc: FusedTrainContext, phase: int, normals: bool = False):
         R, dev = rays_o.shape[0], rays_o.device
         b = tc.buffers(R, phase, dev)
         rgb = torch.empty(R, 3, dtype=torch.float32, device=dev)
@@ -750,12 +750,23 @@ class _FusedTrainStep(torch.autograd.Function):
         with torch.cuda.device(dev):
             _call(_L().perf_train_forward, C.byref(a), _p(rays_o), _p(rays_d), R, phase, C.byref(cb), _stream())
         tc.generation += 1
-        ctx.tc, ctx.phase, ctx.b, ctx.generation = tc, phase, b, tc.generation
+        ctx.tc, ctx.phase, ctx.b, ctx.generation, ctx.normals = tc, phase, b, tc.generation, normals
         ctx.save_for_backward(rays_o, rays_d, jitter, bg_noise, dist, op)
+        if normals:
+            layout = _fixed_layout(tc, rays_o, rays_d, jitter, b)
+            return rgb, dist, op, b["dl"].clone(), _normals_fwd(tc, b, layout, R, R * tc.n_samples, phase, dev)
         return rgb, dist, op, b["dl"].clone()
 
     @staticmethod
-    def backward(ctx, g_rgb, g_dist, g_op, g_dl):
+    def backward(ctx, g_rgb, g_dist, g_op, g_dl, g_nrm=None):
+        grad = _FusedTrainStep._backward(ctx, g_rgb, g_dist, g_op, g_dl)
+        if g_nrm is not None:
+            rays_o, rays_d, jitter = ctx.saved_tensors[:3]
+            _normals_bwd(ctx.tc, ctx.b, _fixed_layout(ctx.tc, rays_o, rays_d, jitter, ctx.b), g_nrm, grad)
+        return grad, None, None, None, None, None, None, None
+
+    @staticmethod
+    def _backward(ctx, g_rgb, g_dist, g_op, g_dl):
         rays_o, rays_d, jitter, bg_noise, dist, op = ctx.saved_tensors
         tc, phase, b = ctx.tc, ctx.phase, ctx.b
         if ctx.generation != tc.generation:
@@ -788,12 +799,12 @@ class _FusedTrainStep(torch.autograd.Function):
                       _stream(), launches=2)
                 _call(_L().perf_hashgrid_bwd_rays_coarse, tc.grid.c(), aabb, _p(rays_o), _p(rays_d), _p(jitter), R, S, tc.near, tc.far,
                       _p(dfeat), _p(d_table), _stream())
-            return grad, None, None, None, None, None, None
+            return grad
         _, dfeat = mlp_backward_half(mlp, half[:mlp.n_params], b["feat"], b["h1"], b["h2"], dz, grad_out=grad[:mlp.n_params])
         with torch.cuda.device(dev):
             _call(_L().perf_hashgrid_bwd_rays, tc.grid.c(), aabb, _p(rays_o), _p(rays_d), _p(jitter), R, S, tc.near, tc.far,
                   _p(dfeat), _p(d_table), _stream(), launches=2)
-        return grad, None, None, None, None, None, None
+        return grad
 
 
 class _FusedPackedTrainStep(torch.autograd.Function):
@@ -808,7 +819,7 @@ class _FusedPackedTrainStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, params, rays_o, rays_d, offsets, ray_indices, t_starts, t_ends, bg_noise, tc: FusedTrainContext, phase: int,
-                early_stop_eps: float, n_dev):
+                early_stop_eps: float, n_dev, normals: bool = False):
         R, N, dev = rays_o.shape[0], t_starts.shape[0], rays_o.device
         geo = phase == _lib.PERF_PHASE_GEO
         b = tc.packed_buffers(R, N, phase, dev)
@@ -822,10 +833,20 @@ class _FusedPackedTrainStep(torch.autograd.Function):
                   _lib.PERF_FLAG_TRAINING, _p(bg_noise), _p(b["w"]), _p(b["T"]), _p(rgb), _p(dist), _p(op), _p(b["dacc"]), _p(b["dl"]), _stream())
         ctx.tc, ctx.phase, ctx.b, ctx.n_dev = tc, phase, b, n_dev
         ctx.save_for_backward(offsets, t_starts, t_ends, bg_noise, dist, op)
+        if normals:
+            ctx.layout, ctx.ray_indices = _packed_layout(tc, b, offsets, ray_indices, n_dev, R, N), ray_indices   # keeps the pointer alive
+            return rgb, dist, op, b["dl"].clone(), _normals_fwd(tc, b, ctx.layout, R, N, phase, dev)
         return rgb, dist, op, b["dl"].clone()
 
     @staticmethod
-    def backward(ctx, g_rgb, g_dist, g_op, g_dl):
+    def backward(ctx, g_rgb, g_dist, g_op, g_dl, g_nrm=None):
+        grad = _FusedPackedTrainStep._backward(ctx, g_rgb, g_dist, g_op, g_dl)
+        if g_nrm is not None:
+            _normals_bwd(ctx.tc, ctx.b, ctx.layout, g_nrm, grad)
+        return (grad,) + (None,) * 12
+
+    @staticmethod
+    def _backward(ctx, g_rgb, g_dist, g_op, g_dl):
         offsets, t_starts, t_ends, bg_noise, dist, op = ctx.saved_tensors
         tc, phase, b, n_dev = ctx.tc, ctx.phase, ctx.b, ctx.n_dev
         R, N, dev = op.shape[0], t_starts.shape[0], op.device
@@ -843,11 +864,13 @@ class _FusedPackedTrainStep(torch.autograd.Function):
         with torch.cuda.device(dev):
             _call(_L().perf_hashgrid_bwd_merged, tc.grid.c(), _p(b["x01"]), _p(dfeat), N, _p(n_dev), _p(grad[mlp.n_params:]),
                   _FusedPackedTrainStep.MERGE_LEVELS, _stream(), launches=2)
-        return (grad,) + (None,) * 11
+        return grad
 
 
 def fused_packed_train_step(params, rays_o, rays_d, offsets, ray_indices, t_starts, t_ends, bg_noise, tc: FusedTrainContext, phase: int,
-                            early_stop_eps: float = 1e-4, n_dev: Optional[torch.Tensor] = None):
+                            early_stop_eps: float = 1e-4, n_dev: Optional[torch.Tensor] = None, normals: bool = False):
+    """(rgb, distance, opacity, distloss numerators) of :class:`_FusedPackedTrainStep`; ``normals`` (density phase): also the ray
+    normal [R,3] = sum_i sg(w_i) n_i, whose gradient reaches the density net (:func:`normal_loss`)."""
     rays_o, rays_d = _chk(rays_o, torch.float32, "rays_o"), _chk(rays_d, torch.float32, "rays_d")
     offsets, ray_indices = _chk(offsets, torch.int64, "offsets"), _chk(ray_indices, torch.int64, "ray_indices")
     t_starts, t_ends = _chk(t_starts, torch.float32, "t_starts"), _chk(t_ends, torch.float32, "t_ends")
@@ -856,7 +879,9 @@ def fused_packed_train_step(params, rays_o, rays_d, offsets, ray_indices, t_star
         raise RuntimeError("perf_b200.fused_packed_train_step: offsets must have R + 1 entries")
     if n_dev is not None:
         n_dev = _chk(n_dev, torch.int64, "n_dev")
-    return _FusedPackedTrainStep.apply(params, rays_o, rays_d, offsets, ray_indices, t_starts, t_ends, bg_noise, tc, phase, early_stop_eps, n_dev)
+    _check_normals(normals, phase)
+    return _FusedPackedTrainStep.apply(params, rays_o, rays_d, offsets, ray_indices, t_starts, t_ends, bg_noise, tc, phase, early_stop_eps, n_dev,
+                                       normals)
 
 
 def gather_rows(idx: torch.Tensor, *arrays: torch.Tensor):
@@ -957,10 +982,87 @@ def occ_update(occs: torch.Tensor, cell_idx: Optional[torch.Tensor], occ_new: to
               _p(occ_new), occ_new.numel(), float(ema_decay), float(occ_thre), _p(binaries_u8), _p(workspace), _stream(), launches=3)
 
 
-def fused_train_step(params, rays_o, rays_d, jitter, bg_noise, tc: FusedTrainContext, phase: int):
+def fused_train_step(params, rays_o, rays_d, jitter, bg_noise, tc: FusedTrainContext, phase: int, normals: bool = False):
+    """(rgb, distance, opacity, distloss numerators) of :class:`_FusedTrainStep`; ``normals`` (density phase): also the ray normal
+    [R,3] = sum_i sg(w_i) n_i, whose gradient reaches the density net (:func:`normal_loss`)."""
     rays_o, rays_d = _chk(rays_o, torch.float32, "rays_o"), _chk(rays_d, torch.float32, "rays_d")
     jitter, bg_noise = _chk(jitter, torch.float32, "jitter"), _chk(bg_noise, torch.float32, "bg_noise")
-    return _FusedTrainStep.apply(params, rays_o, rays_d, jitter, bg_noise, tc, phase)
+    _check_normals(normals, phase)
+    return _FusedTrainStep.apply(params, rays_o, rays_d, jitter, bg_noise, tc, phase, normals)
+
+
+# ------------------------------------------------------------------ normal-consistency loss (density phase)
+def _check_normals(normals: bool, phase: int):
+    if normals and phase != _lib.PERF_PHASE_GEO:
+        raise ValueError("perf_b200: training normals belong to the density phase (phase=PERF_PHASE_GEO)")
+
+
+def _fixed_layout(tc: FusedTrainContext, rays_o, rays_d, jitter, b) -> "_lib.SampleLayout":
+    R = rays_o.shape[0]
+    L = _lib.SampleLayout()
+    L.R, L.N, L.aabb = R, R * tc.n_samples, (C.c_float * 6)(*tc.aabb)
+    L.d_rays_o, L.d_rays_d, L.d_jitter = rays_o.data_ptr(), rays_d.data_ptr(), None if jitter is None else jitter.data_ptr()
+    L.n_samples, L.segments, L.near, L.far = tc.n_samples, int(b["segments"].value), tc.near, tc.far
+    L.d_seg_trans = b["toff"].data_ptr()
+    return L
+
+
+def _packed_layout(tc: FusedTrainContext, b, offsets, ray_indices, n_dev, R: int, N: int) -> "_lib.SampleLayout":
+    L = _lib.SampleLayout()
+    L.R, L.N, L.aabb = R, N, (C.c_float * 6)(*tc.aabb)
+    L.d_x01, L.d_offsets, L.d_ray_indices = b["x01"].data_ptr(), offsets.data_ptr(), ray_indices.data_ptr()
+    L.d_n_dev = None if n_dev is None else n_dev.data_ptr()
+    return L
+
+
+def _normal_buffers(b, N: int, dev):
+    if "nrm" not in b:                 # allocated on the first step that asks for normals, then reused like the other saves
+        b["nrm"] = torch.empty(N, 3, dtype=torch.float32, device=dev)
+        b["rinv"] = torch.empty(N, dtype=torch.float32, device=dev)
+    return b["nrm"], b["rinv"]
+
+
+def _normals_fwd(tc: FusedTrainContext, b, layout, R: int, N: int, phase: int, dev) -> torch.Tensor:
+    nrm, rinv = _normal_buffers(b, N, dev)
+    ray_nrm = torch.empty(R, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_normals_train_fwd, tc.grid.c(), GEO_MLP.c(), _p(tc.geo_half), C.byref(layout), _p(b["h1"]), _p(b["w"]), _p(b["T"]),
+              _p(nrm), _p(rinv), _p(ray_nrm), _stream(), launches=2)
+    return ray_nrm
+
+
+def _normals_bwd(tc: FusedTrainContext, b, layout, g_nrm: torch.Tensor, grad: torch.Tensor) -> None:
+    g_nrm = g_nrm.contiguous().float()
+    with torch.cuda.device(grad.device):
+        _call(_L().perf_normals_train_bwd, tc.grid.c(), GEO_MLP.c(), _p(tc.geo_half), C.byref(layout), _p(b["h1"]), _p(b["w"]), _p(b["T"]),
+              _p(b["nrm"]), _p(b["rinv"]), _p(g_nrm), _p(grad), _stream())
+
+
+class _NormalLoss(torch.autograd.Function):
+    """L_n = mean over valid rays of |N^ - g^|_1 + (1 - N^ . g^) (MonoSDF), ONE kernel that also forms dL_n / dN
+    (include/perfb200.h, perf_normal_loss); backward scales it by the incoming gradient."""
+
+    @staticmethod
+    def forward(ctx, nrm, gt):
+        R, dev = nrm.shape[0], nrm.device
+        loss2 = torch.empty(2, dtype=torch.float32, device=dev)
+        g = torch.empty(R, 3, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _call(_L().perf_normal_loss, _p(_chk(nrm.detach(), torch.float32, "normal")), _p(_chk(gt, torch.float32, "gt_normal")), R,
+                  _p(loss2), _p(g), _stream())
+        ctx.save_for_backward(g)
+        return loss2[0], loss2[1].detach()
+
+    @staticmethod
+    def backward(ctx, go, _g1):
+        (g,) = ctx.saved_tensors
+        return g * go, None
+
+
+def normal_loss(nrm: torch.Tensor, gt: torch.Tensor):
+    """(L_n, number of valid rays) of the ray normals ``nrm`` [R,3] against the supervision normals ``gt`` [R,3]; differentiable
+    w.r.t. ``nrm``.  A ray counts when |gt| > 0.5 and |nrm| > 1e-6; both outputs stay on the device."""
+    return _NormalLoss.apply(nrm, gt.reshape(nrm.shape))
 
 
 # ------------------------------------------------------------------ optimiser

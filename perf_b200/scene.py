@@ -157,10 +157,16 @@ class RaySupervision:
         self.use_default_generator = False
 
     @staticmethod
-    def from_panorama(pose, rgb: torch.Tensor, distance: torch.Tensor, seed: int = 0) -> "RaySupervision":
+    def from_panorama(pose, rgb: torch.Tensor, distance: torch.Tensor, seed: int = 0, normals: Optional[torch.Tensor] = None) -> "RaySupervision":
+        """``normals`` [h, w, 3] (optional): the panorama's normal map in its camera frame, pointing toward the camera (PeRF's
+        ``<image>_ref_normal.npy``); stored rotated into the world frame by ``pose[:3, :3]``, like the ray directions."""
         h, w = distance.shape[:2]
         rays = gen_pano_rays(pose, h, w, device=rgb.device)
-        pool = RaySupervision(Rays(rays.o.reshape(-1, 3), rays.d.reshape(-1, 3)), rgb.reshape(-1, 3).float(), distance.reshape(-1, 1).float(), seed=seed)
+        if normals is not None:
+            rot = torch.as_tensor(pose, dtype=torch.float32).to(rgb.device)[:3, :3]
+            normals = (normals.reshape(-1, 3).float().to(rgb.device) @ rot.t()).contiguous()
+        pool = RaySupervision(Rays(rays.o.reshape(-1, 3), rays.d.reshape(-1, 3)), rgb.reshape(-1, 3).float(), distance.reshape(-1, 1).float(),
+                              normals=normals, seed=seed)
         # Morton (Z-order) code of the pixel: a batch sorted by it puts rays that are neighbours on the
         # sphere into the same warp, so their hash-grid gathers share cache lines at the coarse levels.
         # The batch is the same multiset of rays torch.randint drew (sup_info.py:253-257); only its order changes.
@@ -468,10 +474,11 @@ class NeRFScene:
         distance = self.render(rays, query_keys=["distance"])["distance"].squeeze()
         return sup_pool.pano_visibility_mask(rays, distance)
 
-    def _render_once_fused(self, rays: Rays, geo_inference: bool, app_inference: bool):
+    def _render_once_fused(self, rays: Rays, geo_inference: bool, app_inference: bool, normals: bool = False):
         """Training-mode render as ONE forward kernel; gradients reach the network that is not in
         inference mode.  Same outputs as the modular path except the per-sample tensors: instead of
-        `weights/t_starts/t_ends/ray_indices` it returns `dist_loss` (= flatten_eff_distloss)."""
+        `weights/t_starts/t_ends/ray_indices` it returns `dist_loss` (= flatten_eff_distloss).  ``normals`` (density phase): also
+        `normal` [R,3] = sum_i sg(w_i) n_i, differentiable w.r.t. the density net (the normal-consistency loss)."""
         from . import _lib
         rays_o, rays_d = rays.collapse()
         R, dev = rays_o.shape[0], rays_o.device
@@ -496,30 +503,35 @@ class NeRFScene:
                 ri, ts, te, offsets, n_dev = ops.occ_sample_static(est.binaries[0], est._aabb_list(), rays_o.float().contiguous(),
                                                                    rays_d.float().contiguous(), 0.0, 1.5, self.OCC_STEP,
                                                                    jitter if self.nerf.training else None, static)
-                rgb, dist, op, dl = ops.fused_packed_train_step(param, rays_o.float(), rays_d.float(), offsets, ri, ts, te, noise, tc, phase, 1e-4, n_dev=n_dev)
+                out = ops.fused_packed_train_step(param, rays_o.float(), rays_d.float(), offsets, ri, ts, te, noise, tc, phase, 1e-4, n_dev=n_dev,
+                                                  normals=normals)
+                rgb, dist, op, dl = out[:4]
                 n_rays = (ri[(n_dev - 1).clamp(min=0)] + 1).float().reshape(())       # flatten_eff_distloss: ray_id.max() + 1
                 return {"is_valid": True, "rgb": rgb, "distance": dist, "opacities": op, "dist_loss": _Lazy(lambda: dl.sum() / n_rays),
-                        "dist_loss_rays": dl, "dist_loss_inv_n": 1.0 / n_rays}
+                        "dist_loss_rays": dl, "dist_loss_inv_n": 1.0 / n_rays, **({"normal": out[4]} if normals else {})}
             ri, ts, te = ops.occ_sample(est.binaries[0], est._aabb_list(), rays_o.float().contiguous(), rays_d.float().contiguous(),
                                         0.0, 1.5, self.OCC_STEP, jitter if self.nerf.training else None)
             if ri.numel() <= 0:                                              # nerf_renderer.py:156-162
                 z = lambda c: torch.zeros(R, c, device=dev)
                 return {"is_valid": False, "rgb": z(3), "distance": z(1), "opacities": z(1), "dist_loss": torch.zeros((), device=dev)}
-            rgb, dist, op, dl = ops.fused_packed_train_step(param, rays_o.float(), rays_d.float(), ops.occ_sample.last_offsets, ri, ts, te,
-                                                            noise, tc, phase, 1e-4)
+            out = ops.fused_packed_train_step(param, rays_o.float(), rays_d.float(), ops.occ_sample.last_offsets, ri, ts, te,
+                                              noise, tc, phase, 1e-4, normals=normals)
+            rgb, dist, op, dl = out[:4]
             n_rays = (ri[-1] + 1).float()                                    # flatten_eff_distloss: ray_id.max() + 1
             return {"is_valid": True, "rgb": rgb, "distance": dist, "opacities": op, "dist_loss": _Lazy(lambda: dl.sum() / n_rays),
-                    "dist_loss_rays": dl, "dist_loss_inv_n": 1.0 / n_rays, "n_samples": int(ri.numel())}
-        rgb, dist, op, dl = ops.fused_train_step(param, rays_o, rays_d, jitter, noise, tc, phase)
+                    "dist_loss_rays": dl, "dist_loss_inv_n": 1.0 / n_rays, "n_samples": int(ri.numel()),
+                    **({"normal": out[4]} if normals else {})}
+        out = ops.fused_train_step(param, rays_o, rays_d, jitter, noise, tc, phase, normals=normals)
+        rgb, dist, op, dl = out[:4]
         return {"is_valid": True, "rgb": rgb, "distance": dist, "opacities": op, "dist_loss": _Lazy(lambda: dl.sum() / R),
-                "dist_loss_rays": dl, "dist_loss_inv_n": None}
+                "dist_loss_rays": dl, "dist_loss_inv_n": None, **({"normal": out[4]} if normals else {})}
 
     def render_once(self, rays: Rays, query_keys=("rgb",), sampling_requires_grad=False, geo_inference=False, app_inference=False):
         """`nerf.py:101-123` (differentiable path used by the train steps)."""
         rays_o, rays_d = rays.collapse()
         assert len(rays_o.shape) == 2
         if self.fused_train and self.nerf.training and (geo_inference != app_inference) and "weights" not in query_keys:
-            res = self._render_once_fused(rays, geo_inference, app_inference)
+            res = self._render_once_fused(rays, geo_inference, app_inference, normals="normal" in query_keys)
             return {k: (res[k]() if isinstance(res[k], _Lazy) else res[k]) for k in list(query_keys) + ["is_valid"] if k in res}
         res = self.renderer.render(self.nerf, self.estimator, rays_o, rays_d, geo_inference=geo_inference, app_inference=app_inference)
         if (res is None) or (not res["is_valid"]):
@@ -584,14 +596,38 @@ class NeRFScene:
         if self.writer is not None:
             self.writer.add_scalar(tag, value, step)
 
+    def _check_normal_loss(self, sup_pool):
+        """The normal-consistency loss needs the fused step (the modular path's tcnn shim has no input gradients, DESIGN §9) and
+        world-frame supervision normals: a registered panorama's normal map is in its camera frame and SupInfoPool rotates only the
+        ray directions (sup_info.py:95-117), which is the world frame only for translation-only poses (all PeRF registers)."""
+        if not self.fused_train:
+            raise NotImplementedError("normal_loss_weight > 0 needs fused_train=True (the modular path has no input gradients)")
+        infos = getattr(sup_pool, "sup_infos", None)
+        key = (id(sup_pool), len(infos) if infos is not None else -1)
+        if infos is None or getattr(self, "_normals_checked", None) == key:
+            return
+        eye = torch.eye(3)
+        for k, info in enumerate(infos):
+            if float((info.pose[:3, :3].detach().float().cpu() - eye).abs().max()) > 1e-6:
+                raise ValueError(f"normal_loss_weight > 0: panorama {k} is registered with a rotation; its normal map is in the "
+                                 "camera frame and SupInfoPool does not rotate normals, so the loss would compare different frames")
+        self._normals_checked = key
+
     def train_one_step_geo(self, optimizer, sup_pool, pixel_sup_rand_mode="by_all_pixels", progress=0.0):
-        """`nerf.py:186-257`: depth smooth-L1 + ramped distortion loss; colour under no_grad."""
+        """`nerf.py:186-257`: depth smooth-L1 + ramped distortion loss; colour under no_grad.  ``normal_loss_weight`` > 0 adds the
+        normal-consistency loss against the batch's supervision normals (DESIGN §4)."""
         conf, eps, loss = self.train_conf, 1e-7, 0.
+        w_normal = float(conf.get("normal_loss_weight", 0.))
+        use_normal = w_normal > eps
+        if use_normal:
+            self._check_normal_loss(sup_pool)
         optimizer.zero_grad()
-        rays, gt_colors, gt_depths, _ = sup_pool.rand_ray_color_data(self._local_batch(), rand_mode=pixel_sup_rand_mode)
+        rays, gt_colors, gt_depths, gt_normals = sup_pool.rand_ray_color_data(self._local_batch(), rand_mode=pixel_sup_rand_mode)
         one_kernel_loss = self.fused_train and conf.density_loss_weight <= eps
         keys = (["rgb", "distance", "dist_loss_rays", "dist_loss_inv_n"] if one_kernel_loss else ["rgb", "distance", "dist_loss"]) if self.fused_train \
             else ["rgb", "distance", "weights", "t_starts", "t_ends", "trans", "ray_indices"]
+        if use_normal:
+            keys = keys + ["normal"]
         res = self.render_once(rays, keys, app_inference=True)
         if (res is None) or (not res["is_valid"]):
             optimizer.step(valid=False)            # no samples on this rank (nerf.py:204-206): still join the exchange
@@ -608,6 +644,10 @@ class NeRFScene:
                                                          w_dl=conf.distortion_loss_weight if use_dl else 0.0)
             self._log("nerf_loss/depth_loss", depth_loss, self.global_iter_step_geo)
             self._log("nerf_loss/dist_loss", dist_loss, self.global_iter_step_geo)
+            if use_normal:
+                normal_loss, _ = ops.normal_loss(res["normal"], gt_normals)
+                loss = loss + normal_loss * w_normal
+                self._log("nerf_loss/normal_loss", normal_loss, self.global_iter_step_geo)
             (loss * self.LOSS_SCALE).backward()
             optimizer.step()
             self.global_iter_step_geo += 1
@@ -629,6 +669,10 @@ class NeRFScene:
         if conf.density_loss_weight > eps:
             rand_pts = (torch.rand(8192, 3, device=self.device) * 2. - 1.) * 0.99
             loss = loss + self.nerf.query_density(rand_pts).mean() * conf.density_loss_weight
+        if use_normal:
+            normal_loss, _ = ops.normal_loss(res["normal"], gt_normals)
+            loss = loss + normal_loss * w_normal
+            self._log("nerf_loss/normal_loss", normal_loss, self.global_iter_step_geo)
         (loss * self.LOSS_SCALE).backward()
         optimizer.step()
         self.global_iter_step_geo += 1

@@ -27,6 +27,16 @@ def box_room_distance(h: int, w: int, half_extents=(0.6, 0.8, 0.45), device="cpu
     return t.min(-1, keepdim=True).values
 
 
+def box_room_normals(h: int, w: int, half_extents=(0.6, 0.8, 0.45), device="cpu") -> torch.Tensor:
+    """[h, w, 3]: the inward unit normal of the box face each pixel sees (it points toward the camera at the origin, the
+    orientation of PeRF's normal maps); camera frame = world frame for the identity pose."""
+    d = pano_directions(h, w, device)
+    ext = torch.tensor(half_extents, device=device)
+    axis = (ext / d.abs().clamp(min=1e-9)).argmin(-1, keepdim=True)
+    n = torch.zeros(h, w, 3, device=device)
+    return n.scatter_(-1, axis, -torch.sign(torch.gather(d, -1, axis)))
+
+
 def smooth_rgb(h: int, w: int, seed: int = 0, device="cpu") -> torch.Tensor:
     """[h, w, 3] in [0,1]: sum of 8 random low-frequency sinusoids of the direction per channel."""
     g = torch.Generator().manual_seed(seed)
