@@ -399,7 +399,7 @@ int perf_normals_train_fwd(const perf_grid_cfg* grid, const perf_mlp_cfg* mlp, c
                            const void* d_h1, const float* d_weights, const float* d_trans,
                            float* d_sample_normal, float* d_inv_norm, float* d_ray_normal, void* stream);
 /* The loss above in one launch: d_loss2 = {L_n, #valid}; d_g_ray_normal [R,3] = dL_n / dN_r (unscaled, 0 on invalid rays).
- * d_ray_normal / d_gt_normal [R,3].  The valid count stays on the device. */
+ * d_ray_normal / d_gt_normal [R,3] (NULL allowed when R = 0: d_loss2 = {0, 0}).  The valid count stays on the device. */
 int perf_normal_loss(const float* d_ray_normal, const float* d_gt_normal, uint64_t R, float* d_loss2, float* d_g_ray_normal, void* stream);
 /* Backward of the ray normals into the density net: with G_r = d_g_ray_normal [R,3] and u = -(I - n n^T)(w_i G_r) / |grad|,
  * v = u / aabb extent (= dL/d grad01), per level dg = sum_d v_d scale s' A_d (the dfeat branch of perf_hashgrid_bwd_bwd_input) and the

@@ -430,7 +430,8 @@ int perf_normals_train_fwd(const perf_grid_cfg* grid, const perf_mlp_cfg* mlp, c
 
 int perf_normal_loss(const float* d_ray_normal, const float* d_gt_normal, uint64_t R, float* d_loss2, float* d_g_ray_normal, void* stream)
 {
-    PERF_CHECK_ARG(d_ray_normal && d_gt_normal && d_loss2 && d_g_ray_normal, "NULL pointer");
+    // a batch without rays has L_n = 0 and no valid ray; its [0,3] arrays may be NULL (an empty tensor's storage)
+    PERF_CHECK_ARG(d_loss2 && (R == 0 || (d_ray_normal && d_gt_normal && d_g_ray_normal)), "NULL pointer");
     normal_loss_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(d_ray_normal, d_gt_normal, R, d_loss2, d_g_ray_normal);
     PERF_LAUNCH_CHECK();
     return PERF_OK;

@@ -4,6 +4,7 @@ the unrounded field, and perf_b200/csrc/normal_loss.cu's __host__ __device__ bod
 ray normals, v = dL/d grad01, dg, the table gradient, P -> dW1 / dw_out, the loss and dL/dN, for both sample layouts, with invalid
 rays, dropped samples and samples without gradient."""
 import ctypes as C
+import dataclasses
 import os
 import subprocess
 
@@ -20,6 +21,10 @@ CSRC = os.path.join(os.path.dirname(HERE), "perf_b200", "csrc")
 OUT = os.path.join(HERE, "_build", "libperf_normal_loss_harness.so")
 # 16 levels (the density net's 32 inputs) on a small table so the fp64 oracle and central differences stay cheap
 GRID = OGrid(n_levels=16, log2_hashmap_size=9, base_resolution=2, per_level_scale=1.35)
+UNIT = (-1., -1., -1., 1., 1., 1.)
+# boxes whose extents differ per axis, so that a division by the wrong axis' extent shows: one takes div_uniform's 3-FMA path,
+# the other has an x extent with an all-ones significand (2 - 2^-23 in fp32), where div_uniform falls back to the IEEE division
+BOXES = {"skew": (-0.7, -1.3, -0.9, 1.1, 0.8, 1.4), "allones": (-1., -1., -1., 0.99999988, 1., 2.)}
 _LIB = None
 
 
@@ -58,23 +63,28 @@ def _field(seed=3):
 
 
 class _Case:
-    """A batch in one of the two layouts, with weights / T / h1 that exercise every branch."""
+    """A batch in one of the two layouts, with weights / T / h1 that exercise every branch.  ``field.aabb`` is the box;
+    fixed-S: samples over [near, far], ``segments`` > 1 scales each segment's weights and T by a random start transmittance."""
 
-    def __init__(self, field, layout, R=24, S=12, seed=0):
+    def __init__(self, field, layout, R=24, S=12, seed=0, near=1e-2, far=1.0, segments=1):
         g = torch.Generator().manual_seed(seed)
         self.field, self.layout, self.R = field, layout, R
+        self.aabb = tuple(float(v) for v in field.aabb)
+        self.near, self.far, self.segments = near, far, segments
         self.o = ((torch.rand(R, 3, generator=g) - .5) * .4).numpy().astype(np.float32)
         d = torch.nn.functional.normalize(torch.randn(R, 3, generator=g), dim=-1)
         self.d = d.numpy().astype(np.float32)
         self.jit = torch.rand(R, generator=g).numpy().astype(np.float32)
         if layout == "fixed":
             self.S, self.N = S, R * S
-            step = np.float32(np.float32(1.0) - np.float32(1e-2)) / np.float32(S)
+            n32, f32 = np.float32(near), np.float32(far)
+            step = np.float32(f32 - n32) / np.float32(S)
             k = np.arange(S, dtype=np.float32)[:, None]
-            ts = np.float32(1e-2) + (k + self.jit[None]) * step
-            te = np.float32(1e-2) + (k + np.float32(1) + self.jit[None]) * step
+            ts = n32 + (k + self.jit[None]) * step
+            te = n32 + (k + np.float32(1) + self.jit[None]) * step
             pos = self.o[None] + (self.d[None] * (ts + te)[..., None]) * np.float32(0.5)
-            self.x01 = ((pos + np.float32(1)) / np.float32(2)).reshape(-1, 3).astype(np.float32)
+            lo, hi = np.array(self.aabb[:3], np.float32), np.array(self.aabb[3:], np.float32)
+            self.x01 = ((pos - lo) / (hi - lo)).reshape(-1, 3).astype(np.float32)
             self.ray = np.tile(np.arange(R), S)
         else:
             counts = torch.randint(0, 2 * S, (R,), generator=g).numpy()
@@ -93,14 +103,22 @@ class _Case:
         self.h1 = (torch.randn(N, 64, generator=g)).half().numpy()
         self.h1[::3, ::4] = 0                                                    # h1 == 0: outside the mask
         self.params = field.geo_params.half().numpy()
+        # the weight and transmittance along the whole ray, as the oracle sees them (fixed-S segments: times the segment's start T)
+        self.w_ray, self.T_ray = self.w, self.T
+        if segments > 1:
+            self.seg_trans = (torch.rand(segments * R, generator=g) * 0.8 + 0.2).numpy().astype(np.float32)
+            self.seg_trans[5::7] = 0.0                                           # segments behind an opaque one
+            toff = np.repeat(self.seg_trans.reshape(segments, R), S // segments, axis=0).reshape(-1)
+            self.w_ray, self.T_ray = (self.w * toff).astype(np.float32), (self.T * toff).astype(np.float32)
 
     def layout_c(self):
         from perf_b200._lib import SampleLayout
         L = SampleLayout()
-        L.R, L.N, L.aabb = self.R, self.N, (C.c_float * 6)(-1., -1., -1., 1., 1., 1.)
+        L.R, L.N, L.aabb = self.R, self.N, (C.c_float * 6)(*self.aabb)
         if self.layout == "fixed":
             L.d_rays_o, L.d_rays_d, L.d_jitter = self.o.ctypes.data, self.d.ctypes.data, self.jit.ctypes.data
-            L.n_samples, L.segments, L.near, L.far = self.S, 1, 1e-2, 1.0
+            L.n_samples, L.segments, L.near, L.far = self.S, self.segments, self.near, self.far
+            L.d_seg_trans = self.seg_trans.ctypes.data if self.segments > 1 else None
         else:
             L.d_x01, L.d_offsets, L.d_ray_indices = self.x01.ctypes.data, self.offsets.ctypes.data, self.ray_i64.ctypes.data
         return L
@@ -127,7 +145,7 @@ class _Case:
 
     def oracle(self):
         W1, w_out, table = nlo.field_terms(self.field, mixed=True)
-        return nlo.forward(self.field, W1, w_out, table, torch.from_numpy(self.x01), torch.from_numpy(self.w), torch.from_numpy(self.T),
+        return nlo.forward(self.field, W1, w_out, table, torch.from_numpy(self.x01), torch.from_numpy(self.w_ray), torch.from_numpy(self.T_ray),
                            torch.from_numpy(self.ray).long(), self.R, mask=torch.from_numpy(self.h1).float() > 0, mixed=True)
 
 
@@ -142,7 +160,21 @@ def _close(got, want, rtol=2e-5):
 @pytest.mark.parametrize("layout", ["fixed", "packed"])
 def test_host_bodies_match_oracle(layout):
     field = _field()
-    case = _Case(field, layout)
+    _check_host_bodies(field, _Case(field, layout))
+
+
+@pytest.mark.parametrize("box,layout,segments", [(b, l, 1) for b in BOXES for l in ("fixed", "packed")] + [("unit", "fixed", 4), ("skew", "fixed", 4)])
+def test_host_bodies_match_oracle_in_box(box, layout, segments):
+    """The same bodies in boxes whose per-axis extents differ (the world gradient is grad01 / ext per axis; PeRF's [-1,1]^3 box
+    cancels ext out of n, r and v), with rays long enough to leave the box, and fixed-S batches cut into 4 segments."""
+    field = dataclasses.replace(_field(), aabb=torch.tensor(UNIT if box == "unit" else BOXES[box]))
+    case = _Case(field, layout, far=2.5, segments=segments)
+    if layout == "fixed":
+        assert bool(((case.x01 <= 0) | (case.x01 >= 1)).any(-1).any())                 # some samples leave the box
+    _check_host_bodies(field, case)
+
+
+def _check_host_bodies(field, case):
     case.host_fwd()
     t = case.oracle()
     live = t["r"] > 0
@@ -164,7 +196,7 @@ def test_host_bodies_match_oracle(layout):
     # backward given G: v, dg, the table gradient and dW1 / dw_out
     Gt = torch.from_numpy(G).double()
     dparams, v, dg = case.host_bwd(G)
-    want = nlo.backward_terms(field, torch.from_numpy(case.x01), torch.from_numpy(case.w), torch.from_numpy(case.T),
+    want = nlo.backward_terms(field, torch.from_numpy(case.x01), torch.from_numpy(case.w_ray), torch.from_numpy(case.T_ray),
                               torch.from_numpy(case.ray).long(), case.R, Gt, mask=torch.from_numpy(case.h1).float() > 0)
     _close(v, want["v"], rtol=1e-5)
     _close(dg, want["dg"], rtol=1e-5)
