@@ -231,6 +231,38 @@ int perf_fields_packed_normals(const perf_render_args* args, const float* d_rays
                                const float* d_t_starts, const float* d_t_ends, uint64_t N, const int64_t* d_n_dev /* nullable */,
                                float* d_sigma, void* d_rgb_half4, float* d_x01, float* d_normal, void* stream);
 
+/* ---- both fields off the rays: on a lattice and at arbitrary points (eval mode, the kernel body of perf_fields_packed
+ * phase 0; the flags of the normals entry points above return PERF_EUNSUPPORTED).  args: grid / tables / weights / aabb.
+ * Replaces NGPNeRF.query_density / query_rgb on torch-built positions (ngp_nerf.py:136-162) for mesh extraction. */
+/* sigma [nx, ry, rz] fp32 at lattice nodes (i, j, k), i in [x0, x0 + nx), of the rx x ry x rz lattice spanning the box, faces
+ * included: x01_d = i_d / (r_d - 1) (one fp32 division, no world round trip), selector 0 < x01 < 1 strict -- face nodes are
+ * exactly 0.  d_sigma[((i - x0) * ry + j) * rz + k] (x slowest, the occupancy grid's layout).  r_d >= 2 and rx ry rz < 2^31,
+ * else PERF_EINVAL. */
+int perf_fields_lattice(const perf_render_args* args, const int* h_res3, int x0, int nx, float* d_sigma, void* stream);
+/* d_x [N,3] world points: x01 = (x - aabb_min) / ext as perf_fields_packed normalises, the renderer's selector.
+ * d_sigma [N], d_rgb_half4 [N,4] fp16 (4th lane unused), d_normal [N,3] (nullable) = the sample normal defined above. */
+int perf_fields_points(const perf_render_args* args, const float* d_x, uint64_t N, float* d_sigma, void* d_rgb_half4,
+                       float* d_normal /* nullable */, void* stream);
+
+/* ---- surface extraction: marching tetrahedra on the Freudenthal decomposition of a density lattice d_sigma [rx, ry, rz] fp32
+ * (x slowest; any grid of that layout, e.g. perf_fields_lattice's or the occupancy grid).  Node (i,j,k) is inside iff
+ * sigma > threshold.  Each cube splits into the 6 tets 000, e_a, e_a + e_b, 111 (one per axis permutation (a, b, c), in the order
+ * xyz xzy yxz yzx zxy zyx); each node owns the 7 positive edges e = +x +y +z +xy +xz +yz +xyz (0..6), and an edge crosses when
+ * it lies in the lattice and exactly one end is inside.
+ * perf_mesh_count: d_vcount [n] uint8 = crossing edges of the node (<= 7), d_fcount [n] uint8 = triangles of the cube whose
+ * minimum corner is the node (<= 12; 0 on the far faces).  The caller builds exclusive int32 scans d_voff / d_foff of both
+ * (totals V, F < 2^31) and allocates d_vertices [V,3] fp32 (world), d_faces [F,3] int32.
+ * perf_mesh_write: vertex of edge (p, e) = d_voff[p] + popc(mask(p) & ((1 << e) - 1)); with b the edge's other end,
+ *   t = (threshold - sigma_p) / (sigma_b - sigma_p), x01_d = i_d / (r_d - 1) (+ t * ((i_d + 1) / (r_d - 1) - x01_d) along
+ *   the edge's axes), world_d = aabb_min_d + x01_d * (aabb_max_d - aabb_min_d), each step one rounded fp32 operation;
+ * the cube's triangles from d_foff[p] on, tet by tet; each is oriented so that its normal (v1 - v0) x (v2 - v0) points from the
+ * inside to the outside (along -grad sigma of the tet's linear interpolant: the rendered normal's sense); a quad case splits
+ * along the diagonal between its edges (a,c) and (b,d) (inside a < b).  The output order is fixed by the scans: repeated runs
+ * are byte-identical.  r_d >= 2 and rx ry rz < 2^31, else PERF_EINVAL. */
+int perf_mesh_count(const float* d_sigma, const int* h_res3, float threshold, uint8_t* d_vcount, uint8_t* d_fcount, void* stream);
+int perf_mesh_write(const float* d_sigma, const int* h_res3, float threshold, const float* h_aabb6, const int32_t* d_voff,
+                    const int32_t* d_foff, float* d_vertices, int32_t* d_faces, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

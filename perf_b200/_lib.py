@@ -84,6 +84,10 @@ SIGNATURES = {
     "perf_render_pano_normals": (i32, [P(RenderArgs), P(f32), i32, i32, i32, i32, vp, vp]),
     "perf_render_rays_normals": (i32, [P(RenderArgs), vp, vp, u64, vp, vp]),
     "perf_fields_packed_normals": (i32, [P(RenderArgs), vp, vp, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_fields_lattice": (i32, [P(RenderArgs), P(i32), i32, i32, vp, vp]),
+    "perf_fields_points": (i32, [P(RenderArgs), vp, u64, vp, vp, vp, vp]),
+    "perf_mesh_count": (i32, [vp, P(i32), f32, vp, vp, vp]),
+    "perf_mesh_write": (i32, [vp, P(i32), f32, P(f32), vp, vp, vp, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_hashgrid_bwd_rays": (i32, [P(GridCfg), P(f32), vp, vp, vp, u64, u32, f32, f32, vp, vp, vp]),

@@ -1046,6 +1046,78 @@ __global__ void __launch_bounds__(WG_MAX * TILE, 1) packed_fields_kernel(const _
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// probe_fields_kernel: both fields at positions no ray produces, the eval_fields body of packed_fields_kernel phase 0.
+// LATTICE (perf_fields_lattice): the nodes of an rx x ry x rz lattice spanning the box, x01_d = i_d / (r_d - 1) exactly
+// (no world round trip), sigma only.  A tile is a BRICK of 4 x 4 x 8 nodes (warp w = x plane w of the brick, its lanes
+// 4 y rows x 8 z nodes, z fastest), so the corners a warp gathers at a fine level come from a few neighbouring cells,
+// not from one long run along z.  Otherwise (perf_fields_points): N world points, normalised with div_uniform as the packed kernel
+// does; sigma, fp16 colour and (NORMAL) the sample normal.
+struct ProbeArgs {
+    const float* x;               // [N,3] world points (points)
+    uint64_t     N;               // points, or the slab's x planes nx (LATTICE)
+    int          r[3];            // lattice resolution (LATTICE)
+    int          x0;              // first x plane of the slab (LATTICE)
+    uint32_t     bx, by, bz;      // bricks per axis of the slab (LATTICE)
+    float*       sigma;           // [N] (points) or the slab [nx, ry, rz] (LATTICE)
+    __half*      rgb;             // [N,4] fp16 (points)
+    float*       normal;          // [N,3] (NORMAL)
+};
+constexpr int BRICK_X = 4, BRICK_Y = 4, BRICK_Z = 8;
+static_assert(BRICK_X * BRICK_Y * BRICK_Z == TILE && BRICK_Y * BRICK_Z == 32, "a brick is one tile, one x plane per warp");
+
+// A CTA is blockDim.x / 128 warpgroups with one tile loop each, as in render_march_kernel.
+template <int NDENSE, bool NORMAL, bool LATTICE>
+__global__ void __launch_bounds__(WG_MAX * TILE, 1) probe_fields_kernel(const __grid_constant__ RenderArgs a, const ProbeArgs p)
+{
+    static_assert(!(NORMAL && LATTICE), "the lattice kernel writes sigma only");
+    using L = MarchLayout<false, 0, false, NORMAL>;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x / TILE, 0), nwg = blockDim.x / TILE;   // warp-uniform: see render_march_kernel
+    uint8_t* wgs; const RenderSmem sm = field_smem<L>(smem, wg, wgs);
+    const int tid = threadIdx.x % TILE;
+    stage_weights_bulk<L>(smem);                     // the weight operand images, one bulk copy
+    const uint64_t n_tiles = LATTICE ? (uint64_t)p.bx * p.by * p.bz : (p.N + TILE - 1) / TILE;
+    const float rext0 = __frcp_rn(a.aabb_ext[0]), rext1 = __frcp_rn(a.aabb_ext[1]), rext2 = __frcp_rn(a.aabb_ext[2]);
+    for (uint64_t tile = (uint64_t)blockIdx.x * nwg + wg; tile < n_tiles; tile += (uint64_t)gridDim.x * nwg) {
+        bool valid;
+        uint64_t n;                                   // output row
+        float x = 0.5f, y = 0.5f, z = 0.5f;
+        if constexpr (LATTICE) {
+            const uint32_t bzi = (uint32_t)(tile % p.bz), byi = (uint32_t)((tile / p.bz) % p.by), bxi = (uint32_t)(tile / ((uint64_t)p.bz * p.by));
+            const int li = (int)(bxi * BRICK_X) + (tid >> 5);                       // plane inside the slab
+            const int j = (int)(byi * BRICK_Y) + ((tid >> 3) & 3), k = (int)(bzi * BRICK_Z) + (tid & 7);
+            const int i = p.x0 + li;
+            valid = li < (int)p.N && j < p.r[1] && k < p.r[2];
+            n = ((uint64_t)li * p.r[1] + j) * p.r[2] + k;
+            if (valid) {
+                x = __fdiv_rn((float)i, (float)(p.r[0] - 1));
+                y = __fdiv_rn((float)j, (float)(p.r[1] - 1));
+                z = __fdiv_rn((float)k, (float)(p.r[2] - 1));
+            }
+        } else {
+            n = tile * TILE + tid;
+            valid = n < p.N;
+            if (valid) {
+                x = div_uniform(__fsub_rn(p.x[3 * n], a.aabb_min[0]), a.aabb_ext[0], rext0, a.div_generic != 0u);
+                y = div_uniform(__fsub_rn(p.x[3 * n + 1], a.aabb_min[1]), a.aabb_ext[1], rext1, a.div_generic != 0u);
+                z = div_uniform(__fsub_rn(p.x[3 * n + 2], a.aabb_min[2]), a.aabb_ext[2], rext2, a.div_generic != 0u);
+            }
+        }
+        const bool selector = valid && x > 0.f && x < 1.f && y > 0.f && y < 1.f && z > 0.f && z < 1.f;
+        float sigma, cr, cg, cb, nrm[3];
+        eval_fields<false, NDENSE, 0, L::EVAL, false, NORMAL>(a, sm, x, y, z, selector, tid, sigma, cr, cg, cb, ~0ull, nrm);
+        if (valid) {
+            p.sigma[n] = sigma;
+            if constexpr (!LATTICE) {
+                if constexpr (NORMAL) { p.normal[3 * n] = nrm[0]; p.normal[3 * n + 1] = nrm[1]; p.normal[3 * n + 2] = nrm[2]; }
+                const __half2 c01 = __floats2half2_rn(cr, cg), c2 = __floats2half2_rn(cb, 0.f);
+                *reinterpret_cast<uint2*>(p.rgb + n * 4) = make_uint2(*reinterpret_cast<const uint32_t*>(&c01), *reinterpret_cast<const uint32_t*>(&c2));
+            }
+        }
+    }
+}
+
 static int prepare_weights(const RenderArgs& a, cudaStream_t stream)
 {
     static thread_local int sym_dev = -1; static thread_local float* sym = nullptr;
@@ -1121,6 +1193,12 @@ template <int NDENSE, int SAVE, bool NORMAL = false>
 static int launch_packed(uint64_t n_work, cudaStream_t stream, const RenderArgs& a, const PackedFieldArgs& p)
 {
     return launch_field<packed_fields_kernel<NDENSE, SAVE, NORMAL>, MarchLayout<false, SAVE, false, NORMAL>>(WG_MAX, n_work, stream, a, p);
+}
+
+template <int NDENSE, bool NORMAL, bool LATTICE>
+static int launch_probe(uint64_t n_work, cudaStream_t stream, const RenderArgs& a, const ProbeArgs& p)
+{
+    return launch_field<probe_fields_kernel<NDENSE, NORMAL, LATTICE>, MarchLayout<false, 0, false, NORMAL>>(WG_MAX, n_work, stream, a, p);
 }
 
 // The part of RenderArgs every field kernel needs: level table, packed table and its cell-major copies, weights, aabb and
@@ -1351,6 +1429,53 @@ int perf_fields_packed_normals(const perf_render_args* args, const float* d_rays
     PERF_NORMALS_FLAGS_OK(args);
     return fields_packed(args, d_rays_o, d_rays_d, d_ray_indices, d_t_starts, d_t_ends, N, d_n_dev, 0, d_sigma, d_rgb_half4, d_x01,
                          nullptr, nullptr, nullptr, d_normal, stream);
+}
+
+// ---- fields on a lattice and at points (perfb200.h: perf_fields_lattice, perf_fields_points)
+int perf_fields_lattice(const perf_render_args* args, const int* h_res3, int x0, int nx, float* d_sigma, void* stream)
+{
+    PERF_CHECK_ARG(args && h_res3 && d_sigma, "NULL pointer");
+    PERF_CHECK_ARG(h_res3[0] >= 2 && h_res3[1] >= 2 && h_res3[2] >= 2, "lattice %d x %d x %d: every axis needs >= 2 nodes", h_res3[0], h_res3[1], h_res3[2]);
+    PERF_CHECK_ARG((uint64_t)h_res3[0] * (uint64_t)h_res3[1] * (uint64_t)h_res3[2] < (1ull << 31), "lattice %d x %d x %d has >= 2^31 nodes",
+                   h_res3[0], h_res3[1], h_res3[2]);
+    PERF_CHECK_ARG(x0 >= 0 && nx >= 0 && x0 + nx <= h_res3[0], "x slab [%d, %d + %d) not inside [0, %d)", x0, x0, nx, h_res3[0]);
+    PERF_NORMALS_FLAGS_OK(args);
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    bool fast = false;
+    int rc = init_field_args(args, a, fast); if (rc) return rc;
+    if (nx == 0) return PERF_OK;
+    ProbeArgs p; memset(&p, 0, sizeof(p));
+    p.N = (uint64_t)nx; p.x0 = x0; p.sigma = d_sigma;
+    for (int d = 0; d < 3; ++d) p.r[d] = h_res3[d];
+    p.bx = (uint32_t)((nx + BRICK_X - 1) / BRICK_X); p.by = (uint32_t)((h_res3[1] + BRICK_Y - 1) / BRICK_Y); p.bz = (uint32_t)((h_res3[2] + BRICK_Z - 1) / BRICK_Z);
+    cudaStream_t st = (cudaStream_t)stream;
+    rc = prepare_weights(a, st); if (rc) return rc;
+    const uint64_t n_tiles = (uint64_t)p.bx * p.by * p.bz;
+    rc = fast ? launch_probe<4, false, true>(n_tiles, st, a, p) : launch_probe<-1, false, true>(n_tiles, st, a, p);
+    if (rc) return rc;
+    PERF_LAUNCH_CHECK();
+    return PERF_OK;
+}
+
+int perf_fields_points(const perf_render_args* args, const float* d_x, uint64_t N, float* d_sigma, void* d_rgb_half4, float* d_normal, void* stream)
+{
+    PERF_CHECK_ARG(args && (N == 0 || (d_x && d_sigma && d_rgb_half4)), "NULL pointer");
+    PERF_CHECK_ARG((uintptr_t)d_rgb_half4 % 8 == 0, "misaligned buffer");
+    PERF_NORMALS_FLAGS_OK(args);
+    RenderArgs a; memset(&a, 0, sizeof(a));
+    bool fast = false;
+    int rc = init_field_args(args, a, fast); if (rc) return rc;
+    if (N == 0) return PERF_OK;
+    ProbeArgs p; memset(&p, 0, sizeof(p));
+    p.x = d_x; p.N = N; p.sigma = d_sigma; p.rgb = (__half*)d_rgb_half4; p.normal = d_normal;
+    cudaStream_t st = (cudaStream_t)stream;
+    rc = prepare_weights(a, st); if (rc) return rc;
+    const uint64_t n_tiles = (N + TILE - 1) / TILE;
+    if (d_normal != nullptr) rc = fast ? launch_probe<4, true, false>(n_tiles, st, a, p) : launch_probe<-1, true, false>(n_tiles, st, a, p);
+    else rc = fast ? launch_probe<4, false, false>(n_tiles, st, a, p) : launch_probe<-1, false, false>(n_tiles, st, a, p);
+    if (rc) return rc;
+    PERF_LAUNCH_CHECK();
+    return PERF_OK;
 }
 #undef PERF_NORMALS_FLAGS_OK
 

@@ -617,6 +617,73 @@ def render_pano(packed_table, geo_mlp_half, app_mlp_half, pose, H: int, W: int, 
     return rgb, dist, op
 
 
+# ------------------------------------------------------------------ fields off the rays, surface extraction
+def _res3(resolution):
+    r = (int(resolution),) * 3 if isinstance(resolution, int) else tuple(int(v) for v in resolution)
+    if len(r) != 3:
+        raise ValueError(f"resolution must be an int or (rx, ry, rz), got {resolution!r}")
+    return r
+
+
+def fields_lattice(packed_table, geo_mlp_half, app_mlp_half, resolution, aabb=(-1., -1., -1., 1., 1., 1.), grid: GridConfig = PERF_GRID,
+                   x0: int = 0, nx: Optional[int] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sigma [nx, ry, rz] fp32 at the nodes of the rx x ry x rz lattice spanning ``aabb`` (faces included, x slowest), x planes
+    [x0, x0 + nx) (default: all): ``perf_fields_lattice``.  Node (i, j, k) sits at x01 = (i, j, k) / (r - 1); face nodes are 0."""
+    r = _res3(resolution)
+    nx = r[0] - x0 if nx is None else int(nx)
+    dev = packed_table.device
+    if out is None:
+        out = torch.empty(max(nx, 0), r[1], r[2], dtype=torch.float32, device=dev)
+    elif out.shape != (nx, r[1], r[2]) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError(f"fields_lattice: out must be a contiguous fp32 [{nx}, {r[1]}, {r[2]}] tensor")
+    a = _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, 1, 0.0, 1.0, False, False, None, None, out, out, None, grid)
+    with torch.cuda.device(dev):
+        _call(_L().perf_fields_lattice, C.byref(a), (C.c_int * 3)(*r), int(x0), int(nx), _p(out), _stream(), launches=2)
+    return out
+
+
+def fields_points(packed_table, geo_mlp_half, app_mlp_half, x, aabb=(-1., -1., -1., 1., 1., 1.), grid: GridConfig = PERF_GRID,
+                  normals: bool = False):
+    """Both fields at world points x [N,3] -> (sigma [N] fp32, rgb [N,3] fp16) and with ``normals`` the sample normal [N,3]
+    (unit, 0 outside the box; include/perfb200.h defines it): ``perf_fields_points``."""
+    x = _chk(x, torch.float32, "x").reshape(-1, 3)
+    N, dev = x.shape[0], x.device
+    sigma = torch.empty(N, dtype=torch.float32, device=dev)
+    c16 = torch.empty(N, 4, dtype=torch.float16, device=dev)
+    nrm = torch.empty(N, 3, dtype=torch.float32, device=dev) if normals else None
+    if N:
+        a = _render_args(packed_table, geo_mlp_half, app_mlp_half, aabb, 1, 0.0, 1.0, False, False, None, None, sigma, sigma, None, grid)
+        with torch.cuda.device(dev):
+            _call(_L().perf_fields_points, C.byref(a), _p(x), N, _p(sigma), _p(c16), _p(nrm), _stream(), launches=2)
+    return (sigma, c16[:, :3], nrm) if normals else (sigma, c16[:, :3])
+
+
+def marching_tets(sigma: torch.Tensor, threshold: float, aabb=(-1., -1., -1., 1., 1., 1.)):
+    """Surface {sigma = threshold} of a density lattice sigma [rx, ry, rz] (x slowest; the lattice spans ``aabb``, faces
+    included) by marching tetrahedra: ``perf_mesh_count``, two exclusive scans, ``perf_mesh_write``.  Returns (vertices [V,3]
+    fp32 world, faces [F,3] int32), triangles facing away from high sigma.  One host read (the two totals)."""
+    sigma = _chk(sigma, torch.float32, "sigma")
+    if sigma.dim() != 3:
+        raise ValueError(f"marching_tets: sigma must be [rx, ry, rz], got {tuple(sigma.shape)}")
+    dev, n = sigma.device, sigma.numel()
+    res3 = (C.c_int * 3)(*[int(v) for v in sigma.shape])
+    vc = torch.empty(n, dtype=torch.uint8, device=dev)
+    fc = torch.empty(n, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_mesh_count, _p(sigma), res3, float(threshold), _p(vc), _p(fc), _stream())
+        vinc, finc = torch.cumsum(vc, 0, dtype=torch.int64), torch.cumsum(fc, 0, dtype=torch.int64)
+        V, F = (int(v) for v in torch.stack([vinc[-1], finc[-1]]).tolist())
+        if V >= 2 ** 31 or F >= 2 ** 31:
+            raise RuntimeError(f"marching_tets: {V} vertices / {F} faces do not fit int32 indices")
+        verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
+        faces = torch.empty(F, 3, dtype=torch.int32, device=dev)
+        if V:
+            voff, foff = (vinc - vc).to(torch.int32), (finc - fc).to(torch.int32)
+            a6 = (C.c_float * 6)(*[float(v) for v in aabb])
+            _call(_L().perf_mesh_write, _p(sigma), res3, float(threshold), a6, _p(voff), _p(foff), _p(verts), _p(faces), _stream())
+    return verts, faces
+
+
 # ------------------------------------------------------------------ fused training step
 class FusedTrainContext:
     """Everything one fused training step needs besides the rays: the fp16 shadows / gather table,

@@ -72,6 +72,8 @@ class CoreRunner:
             self.train()
         elif mode == "render_dense":
             self.render_dense()
+        elif mode == "export_mesh":
+            self.export_mesh()
         else:
             raise ValueError(f"mode={mode!r}")
 
@@ -197,6 +199,23 @@ class CoreRunner:
         if self.is_main and write and frames:
             self._write_video(pjoin(out_dir, "video.mp4"), frames)
         return frames
+
+    def export_mesh(self, resolution=None, threshold=None):
+        """The fitted scene as a triangle mesh with vertex colours and normals (``NeRFScene.extract_mesh``), written by rank 0
+        to ``<exp_dir>/mesh/mesh_<res>.ply`` (binary PLY); extracted on the calling rank alone.  Like ``render_dense`` it uses
+        the scene as constructed (``is_continue: true`` loads the checkpoint).  Config keys ``mesh_resolution`` (default 512)
+        and ``mesh_threshold`` (default ``mesh.DEFAULT_THRESHOLD``).  Returns (path, mesh) on rank 0, else (None, None)."""
+        from .mesh import write_ply
+        if not self.is_main:
+            return None, None
+        res = int(resolution if resolution is not None else self.conf.get("mesh_resolution", 512))
+        thr = threshold if threshold is not None else self.conf.get("mesh_threshold", None)
+        self.set_eval()
+        mesh = self.scene.extract_mesh(res, None if thr is None else float(thr))
+        os.makedirs(pjoin(self.exp_dir, "mesh"), exist_ok=True)
+        path = pjoin(self.exp_dir, "mesh", "mesh_{}.ply".format(res))
+        write_ply(path, mesh)
+        return path, mesh
 
     @staticmethod
     def _write_video(path, frames, fps=30):
