@@ -263,6 +263,58 @@ int perf_mesh_count(const float* d_sigma, const int* h_res3, float threshold, ui
 int perf_mesh_write(const float* d_sigma, const int* h_res3, float threshold, const float* h_aabb6, const int32_t* d_voff,
                     const int32_t* d_foff, float* d_vertices, int32_t* d_faces, void* stream);
 
+/* ---- mesh decimation: quadric-error (Garland-Heckbert) edge collapse in rounds of independent collapses, down to a target
+ * face count (ops.decimate drives the rounds; csrc/decimate.cu).
+ * Input: d_vertices [V,3] fp32, d_faces [F,3] int32, a closed, consistently oriented, edge-manifold mesh: every directed edge
+ * a -> b of a face appears exactly once, and so does b -> a (perf_decimate_check).  Half-edge (edge id) i = 3f + k runs from
+ * faces[f][k] to faces[f][(k+1) % 3]; each undirected edge is visited once, as its half-edge with u = a < w = b.
+ * Adjacency (rebuilt by the caller every round): d_adj [3F] int32 = the corners 3f + k sorted by vertex faces[f][k], stable
+ * (so ascending face index per vertex), d_adj_off [V + 1] its offsets.  N(v) = the next vertices of v's corners.
+ * Quadrics (fp64, entries 00 01 02 03 11 12 13 22 23 33 of the symmetric 4x4 Q): per face n = (p1 - p0) x (p2 - p0),
+ *   e = (n / |n|, -(n / |n|) . p0), Q_f = (|n| / 2) e e^T (area-weighted; 0 when n . n = 0); Q_v = sum of Q_f over v's faces in
+ *   ascending face index.  A collapse of w into u sets Q_u <- Q_u + Q_w; quadrics are never recomputed.
+ * Placement, Q = Q_u + Q_w = [[A, b], [b^T, c]]: with adj(A) the cofactors, det = A00 adj00 + A01 adj01 + A02 adj02 and
+ *   tr = A00 + A11 + A22, the system is well conditioned iff det > 1e-6 tr^3 (scale-free; a rank-deficient A -- all faces
+ *   coplanar, or a crease -- fails it).  Then s = -adj(A) b / det, rounded to fp32, is used iff |s - m|^2 <= |u - w|^2 with m =
+ *   0.5 (u + w) in fp64.  Otherwise the cheapest of u, w and fp32(m), first in that order on ties.  The error of p is
+ *   (p, 1)^T Q (p, 1) evaluated at the fp32 point; cost = fp32(max(0, error)).  Every fp64 step is one rounded operation in the
+ *   order csrc/decimate.cu writes (dec_place, dec_err), never contracted.
+ * Validity (all must hold): |N(u) n N(w)| = 2; both vertices opposite the edge have valence (incident faces) > 3; no face of
+ *   star(u) u star(w) that survives the collapse flips: its normals (p1 - p0) x (p2 - p0) before and after (u or w moved to
+ *   the placement) have a positive dot product; faces with n . n = 0 before are exempt.
+ * Selection: key = (fp32 bits of cost) << 32 | edge id (int64, >= 0; INT64_MAX = no candidate); m1[v] = min key over the
+ *   candidate edges at v; m2[v] = min of m1 over v and N(v); edge selected iff key == m2[u] == m2[w].  Selected edges have
+ *   pairwise non-adjacent endpoints, so their stars are disjoint.  Integer atomicMin only: order-independent.
+ * Collapse: Q_u += Q_w, u moves to the placement, w dies, the two faces on the edge die, w is replaced by u in its other faces.
+ *   Each collapse removes 2 faces; the caller applies at most ceil((F - target) / 2) collapses, those with the smallest keys.
+ * Compaction keeps the live faces in order and the live vertices in ascending index.  Rounds end when F <= target or a
+ *   round selects nothing.  All of it is deterministic: repeated runs are byte-identical.
+ * V < 2^31 and 3F < 2^31, else PERF_EINVAL. */
+/* d_flags [1] int32, zeroed by the caller, ORed with: 1 a face repeats a vertex, 2 a directed edge appears more than once,
+ * 4 a directed edge has no opposite (open mesh).  Vertex indices must already lie in [0, V). */
+int perf_decimate_check(const int32_t* d_faces, uint64_t F, uint64_t V, const int32_t* d_adj, const int32_t* d_adj_off, int32_t* d_flags,
+                        void* stream);
+/* d_quadrics [V,10] fp64 of the input mesh. */
+int perf_decimate_quadrics(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_adj,
+                           const int32_t* d_adj_off, double* d_quadrics, void* stream);
+/* Per half-edge: d_key [3F] int64 (INT64_MAX unless a candidate with u < w), d_place [3F,3] fp32 (candidates only);
+ * d_vmin [V] int64 = m1, filled by atomicMin into a caller-set INT64_MAX. */
+int perf_decimate_edges(const float* d_vertices, const double* d_quadrics, uint64_t V, const int32_t* d_faces, uint64_t F,
+                        const int32_t* d_adj, const int32_t* d_adj_off, int64_t* d_key, float* d_place, int64_t* d_vmin, void* stream);
+/* d_vmin2 [V] = m2 (the caller copies m1 into it), d_selected [3F] uint8 = 1 for a selected edge (two launches). */
+int perf_decimate_select(const int32_t* d_faces, uint64_t F, uint64_t V, const int64_t* d_key, const int64_t* d_vmin, int64_t* d_vmin2,
+                         uint8_t* d_selected, void* stream);
+/* Collapses the n selected edge ids d_edges in place: d_vertices, d_quadrics, d_faces; clears d_valive [V] / d_falive [F]
+ * (uint8, set to 1 by the caller) of the dead vertices and faces.  n <= F / 2. */
+int perf_decimate_collapse(const int64_t* d_edges, uint64_t n, float* d_vertices, double* d_quadrics, uint64_t V, int32_t* d_faces,
+                           uint64_t F, const int32_t* d_adj, const int32_t* d_adj_off, const float* d_place, uint8_t* d_valive,
+                           uint8_t* d_falive, void* stream);
+/* d_voff / d_foff: exclusive int32 scans of d_valive / d_falive.  Writes the live vertices and quadrics at d_voff and the live
+ * faces, renumbered by d_voff, at d_foff (two launches). */
+int perf_decimate_compact(const float* d_vertices, const double* d_quadrics, uint64_t V, const uint8_t* d_valive, const int32_t* d_voff,
+                          const int32_t* d_faces, uint64_t F, const uint8_t* d_falive, const int32_t* d_foff,
+                          float* d_out_vertices, double* d_out_quadrics, int32_t* d_out_faces, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

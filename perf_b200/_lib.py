@@ -88,6 +88,12 @@ SIGNATURES = {
     "perf_fields_points": (i32, [P(RenderArgs), vp, u64, vp, vp, vp, vp]),
     "perf_mesh_count": (i32, [vp, P(i32), f32, vp, vp, vp]),
     "perf_mesh_write": (i32, [vp, P(i32), f32, P(f32), vp, vp, vp, vp, vp]),
+    "perf_decimate_check": (i32, [vp, u64, u64, vp, vp, vp, vp]),
+    "perf_decimate_quadrics": (i32, [vp, u64, vp, u64, vp, vp, vp, vp]),
+    "perf_decimate_edges": (i32, [vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_decimate_select": (i32, [vp, u64, u64, vp, vp, vp, vp, vp]),
+    "perf_decimate_collapse": (i32, [vp, u64, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_decimate_compact": (i32, [vp, vp, u64, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_hashgrid_bwd_rays": (i32, [P(GridCfg), P(f32), vp, vp, vp, u64, u32, f32, f32, vp, vp, vp]),

@@ -8,7 +8,7 @@ vertices (``perf_fields_points``), and a binary PLY writer.  PeRF's colour field
 """
 from __future__ import annotations
 
-from typing import Sequence, Union
+from typing import Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -24,18 +24,23 @@ DEFAULT_THRESHOLD = 50.0
 
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
-                 normals: bool = True) -> dict:
+                 normals: bool = True, target_faces: Optional[int] = None) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
     density), with ``colors`` ``"colors"`` [V,3] uint8 = round(clip(rgb, 0, 1) * 255) of the fp16 colour, with ``normals``
-    ``"normals"`` [V,3] f32, the unit density-gradient normal (the rendered normal's definition) -- all on the GPU."""
+    ``"normals"`` [V,3] f32, the unit density-gradient normal (the rendered normal's definition) -- all on the GPU.
+    With ``target_faces`` the mesh is first decimated to about that many faces (``ops.decimate``: quadric-error edge
+    collapse, which removes faces where the surface is flat and keeps them where it bends); colours and normals are then the
+    fields' at the decimated vertices."""
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     sigma = ops.fields_lattice(packed, geo_half, app_half, resolution, aabb, PERF_GRID)
     verts, faces = ops.marching_tets(sigma, threshold, aabb)
     del sigma
+    if target_faces is not None:
+        verts, faces = ops.decimate(verts, faces, target_faces)
     out = {"vertices": verts, "faces": faces}
     if colors or normals:
         res = ops.fields_points(packed, geo_half, app_half, verts, aabb, PERF_GRID, normals=normals)

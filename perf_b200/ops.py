@@ -684,6 +684,95 @@ def marching_tets(sigma: torch.Tensor, threshold: float, aabb=(-1., -1., -1., 1.
     return verts, faces
 
 
+_NO_KEY = 2 ** 63 - 1
+_DECIMATE_FLAGS = {1: "a face repeats a vertex", 2: "a directed edge appears more than once", 4: "the mesh is open (an edge has one face)"}
+
+
+def _corner_adjacency(faces: torch.Tensor, V: int):
+    """Corners 3f + k sorted by vertex (stable: ascending face index per vertex) and their [V + 1] offsets."""
+    flat = faces.view(-1)
+    adj = torch.argsort(flat, stable=True).to(torch.int32)
+    off = torch.zeros(V + 1, dtype=torch.int32, device=faces.device)
+    off[1:] = torch.cumsum(torch.bincount(flat, minlength=V), 0)
+    return adj, off
+
+
+def _exclusive(flags: torch.Tensor) -> torch.Tensor:
+    return torch.cumsum(flags, 0, dtype=torch.int32) - flags
+
+
+def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, stats: Optional[list] = None):
+    """Quadric-error edge collapse of a closed, consistently oriented, edge-manifold mesh (vertices [V,3] fp32, faces [F,3]
+    int32; ``marching_tets`` output is one) down to ``target_faces`` faces: rounds of independent collapses
+    (``perf_decimate_*``; include/perfb200.h states the rules).  Returns (vertices [V',3], faces [F',3]) with F' = target - 1 or
+    target, or more when no collapse is left that keeps the mesh manifold and unfolded.  Faces keep their order and
+    orientation, vertices their relative order; repeated runs are byte-identical.  One host read per round.  ``stats``, when a
+    list, receives the number of collapses of every round.  Raises ValueError for a mesh that is not closed and oriented."""
+    if not isinstance(vertices, torch.Tensor) or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"decimate: vertices must be [V, 3], got {getattr(vertices, 'shape', type(vertices))}")
+    if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"decimate: faces must be [F, 3], got {getattr(faces, 'shape', type(faces))}")
+    if isinstance(target_faces, bool) or int(target_faces) != target_faces or target_faces < 0:
+        raise ValueError(f"decimate: target_faces must be an int >= 0, got {target_faces!r}")
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
+    if V >= 2 ** 31 or 3 * F >= 2 ** 31:
+        raise ValueError(f"decimate: {V} vertices / {F} faces: needs V < 2^31 and 3F < 2^31")
+    target = int(target_faces)
+    if F == 0:
+        return vertices.clone(), faces.clone()
+    L = _L()
+    with torch.cuda.device(dev):
+        lo, hi = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
+        if lo < 0 or hi >= V:
+            raise ValueError(f"decimate: face indices span [{lo}, {hi}], outside [0, {V})")
+        adj, off = _corner_adjacency(faces, V)
+        flags = torch.zeros(1, dtype=torch.int32, device=dev)
+        _call(L.perf_decimate_check, _p(faces), F, V, _p(adj), _p(off), _p(flags), _stream())
+        bad = int(flags.item())
+        if bad:
+            raise ValueError("decimate: not a closed, consistently oriented, edge-manifold mesh: "
+                             + "; ".join(m for b, m in _DECIMATE_FLAGS.items() if bad & b))
+        pos, faces = vertices.clone(), faces.clone()
+        quad = torch.empty(V, 10, dtype=torch.float64, device=dev)
+        _call(L.perf_decimate_quadrics, _p(pos), V, _p(faces), F, _p(adj), _p(off), _p(quad), _stream())
+        first = True
+        while F > target:
+            if not first:
+                adj, off = _corner_adjacency(faces, V)
+            first = False
+            key = torch.empty(3 * F, dtype=torch.int64, device=dev)
+            place = torch.empty(3 * F, 3, dtype=torch.float32, device=dev)
+            vmin = torch.full((V,), _NO_KEY, dtype=torch.int64, device=dev)
+            _call(L.perf_decimate_edges, _p(pos), _p(quad), V, _p(faces), F, _p(adj), _p(off), _p(key), _p(place), _p(vmin), _stream())
+            vmin2, sel = vmin.clone(), torch.empty(3 * F, dtype=torch.uint8, device=dev)
+            _call(L.perf_decimate_select, _p(faces), F, V, _p(key), _p(vmin), _p(vmin2), _p(sel), _stream(), launches=2)
+            edges = torch.nonzero(sel).view(-1)                                   # the round's host read
+            n = edges.numel()
+            if n == 0:
+                break
+            need = (F - target + 1) // 2
+            if n > need:
+                edges = edges[torch.argsort(key[edges])[:need]].contiguous()
+                n = need
+            valive = torch.ones(V, dtype=torch.uint8, device=dev)
+            falive = torch.ones(F, dtype=torch.uint8, device=dev)
+            _call(L.perf_decimate_collapse, _p(edges), n, _p(pos), _p(quad), V, _p(faces), F, _p(adj), _p(off), _p(place),
+                  _p(valive), _p(falive), _stream())
+            del key, place, vmin, vmin2, sel, adj, off
+            V2, F2 = V - n, F - 2 * n
+            pos2 = torch.empty(V2, 3, dtype=torch.float32, device=dev)
+            quad2 = torch.empty(V2, 10, dtype=torch.float64, device=dev)
+            faces2 = torch.empty(F2, 3, dtype=torch.int32, device=dev)
+            voff, foff = _exclusive(valive), _exclusive(falive)          # named: a pointer alone does not keep a tensor alive
+            _call(L.perf_decimate_compact, _p(pos), _p(quad), V, _p(valive), _p(voff), _p(faces), F, _p(falive), _p(foff),
+                  _p(pos2), _p(quad2), _p(faces2), _stream(), launches=2)
+            pos, quad, faces, V, F = pos2, quad2, faces2, V2, F2
+            if stats is not None:
+                stats.append(n)
+    return pos, faces
+
+
 # ------------------------------------------------------------------ fused training step
 class FusedTrainContext:
     """Everything one fused training step needs besides the rays: the fp16 shadows / gather table,
