@@ -315,6 +315,41 @@ int perf_decimate_compact(const float* d_vertices, const double* d_quadrics, uin
                           const int32_t* d_faces, uint64_t F, const uint8_t* d_falive, const int32_t* d_foff,
                           float* d_out_vertices, double* d_out_quadrics, int32_t* d_out_faces, void* stream);
 
+/* ---- texture atlas of a triangle mesh (ops.texture_atlas drives it; csrc/texture.cu).  A T x T texture, T a power of two in
+ * [256, 16384]; texel (x, y) (y up: image row T - 1 - y) covers [x, x + 1] x [y, y + 1] in texel units and has the Morton
+ * index m = interleave(x in the even bits, y in the odd bits).
+ * Charts: face f maps affinely onto a right isosceles triangle.  Its right-angle corner k0 is the corner opposite its longest
+ *   edge (|p_{k+2} - p_{k+1}|^2 = (dx dx + dy dy) + dz dz in fp32; the lowest k on a tie); corners k0 + 1 and k0 + 2 (mod 3)
+ *   follow along the legs, so every chart keeps the face's winding (positive signed area in UV, v up).
+ * Cells: a cell is an aligned s x s square, s = 2^j >= 4, at Morton offset o (a multiple of s^2, lower-left corner
+ *   (compact(o), compact(o >> 1))).  Its first face's chart has the right angle at the corner + (0.5, 0.5) and legs L = s - 3
+ *   along +x (k0 + 1) and +y (k0 + 2); its second face's chart is that triangle rotated 180 degrees about the cell's centre.
+ *   Bleed invariant: the 0.5-texel inset and the 4-texel gap between the hypotenuses make every texel whose centre lies within
+ *   Chebyshev distance < 1 of a chart -- every texel a bilinear lookup on the chart reads -- a texel of the chart's face.
+ * Size classes (caller): leg_f = sqrt(2 area_f) (perf_atlas_legs); with the density d (texels per world unit, fp32) the class
+ *   of f is the smallest s = 2^j >= 4 with fp32(leg_f * d) <= s - 3.  Packing sorts the faces by class descending, then face
+ *   index; consecutive faces of a class pair into cells (the last of an odd class alone); cell offsets are the exclusive scan
+ *   of s^2 in that order, so every cell is aligned and the cells tile [0, used) of the Morton curve without gap or overlap.
+ *   d is the result of a bisection over the bit patterns of the non-negative fp32 values, [0, +inf), that keeps "the cells
+ *   fit in T^2 with no class above T" true at its lower end and false at its upper end.
+ * Texels: texel m lies in the last cell whose offset is <= m (binary search); past the last cell it is unused (face -1,
+ *   point 0).  In a chart's frame (right angle at the origin, legs along +a, +b) the texel centre is an integer point; its
+ *   nearest chart point is found in integers (doubled coordinates), the nearer chart of the cell wins (the first on a tie),
+ *   and with beta = fp32(2a' / 2L), gamma = fp32(2b' / 2L) the point is p = (p_k0 + beta (p_k0+1 - p_k0)) + gamma (p_k0+2 -
+ *   p_k0), each step one rounded fp32 operation in that order.
+ * F < 2^29 and V < 2^31, else PERF_EINVAL. */
+/* d_legs [F] fp32: n = (p1 - p0) x (p2 - p0) in fp32, leg = sqrt(sqrt((nx nx + ny ny) + nz nz)), correctly rounded steps. */
+int perf_atlas_legs(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, float* d_legs, void* stream);
+/* d_order [F] int32: the faces in packing order.  h_classes [n_classes, 5] int32, descending side: (first position in d_order,
+ * face count, first cell, Morton offset of the first cell, side), each class starting where the previous one ends.  Writes
+ * d_uv [F,3,2] fp32 (u, v in [0, 1], v up), d_face_rec [F,4] int32 (cell offset, side, half 0/1, right-angle corner k0) and
+ * d_cells [C,4] int32 (offset, side, first face, second face or -1), C = sum of ceil(count / 2). */
+int perf_atlas_layout(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, int size, const int32_t* d_order,
+                      const int32_t* h_classes, int n_classes, float* d_uv, int32_t* d_face_rec, int32_t* d_cells, void* stream);
+/* Texels m in [m0, m0 + n) (m0 + n <= 2^28): d_face [n] int32 (-1 unused) and d_point [n,3] fp32 world sample points. */
+int perf_atlas_texels(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_face_rec,
+                      const int32_t* d_cells, uint64_t C, uint64_t m0, uint64_t n, int32_t* d_face, float* d_point, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

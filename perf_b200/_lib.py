@@ -94,6 +94,9 @@ SIGNATURES = {
     "perf_decimate_select": (i32, [vp, u64, u64, vp, vp, vp, vp, vp]),
     "perf_decimate_collapse": (i32, [vp, u64, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]),
     "perf_decimate_compact": (i32, [vp, vp, u64, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_atlas_legs": (i32, [vp, u64, vp, u64, vp, vp]),
+    "perf_atlas_layout": (i32, [vp, u64, vp, u64, i32, vp, P(i32), i32, vp, vp, vp, vp]),
+    "perf_atlas_texels": (i32, [vp, u64, vp, u64, vp, vp, u64, u64, u64, vp, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_hashgrid_bwd_rays": (i32, [P(GridCfg), P(f32), vp, vp, vp, u64, u32, f32, f32, vp, vp, vp]),

@@ -24,7 +24,7 @@ DEFAULT_THRESHOLD = 50.0
 
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
-                 normals: bool = True, target_faces: Optional[int] = None) -> dict:
+                 normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -32,7 +32,8 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     ``"normals"`` [V,3] f32, the unit density-gradient normal (the rendered normal's definition) -- all on the GPU.
     With ``target_faces`` the mesh is first decimated to about that many faces (``ops.decimate``: quadric-error edge
     collapse, which removes faces where the surface is flat and keeps them where it bends); colours and normals are then the
-    fields' at the decimated vertices."""
+    fields' at the decimated vertices.  With ``texture_size`` the colour field is then baked into a texture atlas of that side
+    (:func:`bake_texture`): ``"uv"`` [F,3,2] and ``"texture"`` [T,T,3] uint8 join the dict."""
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
@@ -45,10 +46,50 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     if colors or normals:
         res = ops.fields_points(packed, geo_half, app_half, verts, aabb, PERF_GRID, normals=normals)
         if colors:
-            out["colors"] = torch.round(res[1].float().clamp(0.0, 1.0) * 255.0).to(torch.uint8)
+            out["colors"] = _rgb8(res[1])
         if normals:
             out["normals"] = res[2]
+    if texture_size is not None:
+        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size))
     return out
+
+
+def _rgb8(rgb16: torch.Tensor) -> torch.Tensor:
+    return torch.round(rgb16.float().clamp(0.0, 1.0) * 255.0).to(torch.uint8)
+
+
+TEXEL_CHUNK = 1 << 24       # texels per perf_atlas_texels / perf_fields_points pass: bounds the working set at 8192^2 and up
+
+
+def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK) -> dict:
+    atlas = ops.texture_atlas(verts, faces, size)
+    T = atlas["size"]
+    image = torch.zeros(T * T, 3, dtype=torch.uint8, device=verts.device)
+    for m0 in range(0, atlas["used"], chunk):
+        n = min(chunk, atlas["used"] - m0)
+        face, point = ops.atlas_texels(verts, faces, atlas, m0, n)
+        rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
+        rgb[face < 0] = 0
+        x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=verts.device))
+        image[(T - 1 - y) * T + x] = rgb
+        del face, point, rgb, x, y
+    return {"uv": atlas["uv"], "texture": image.view(T, T, 3)}
+
+
+@torch.no_grad()
+def bake_texture(nerf, mesh: dict, size: int) -> dict:
+    """``mesh`` (an :func:`extract_mesh` result) with its colour field baked into a ``size`` x ``size`` texture (a power of two
+    in [256, 16384]): adds ``"uv"`` [F,3,2] fp32 (per face corner, v up) and ``"texture"`` [T,T,3] uint8 (row 0 at v = 1).  One
+    right-isosceles chart per face, packed in Z-order (``ops.texture_atlas``); each texel holds round(clip(rgb, 0, 1) * 255)
+    of the field's colour at the point of its face nearest to the texel centre (``ops.atlas_texels`` then
+    ``perf_fields_points``).  Bilinear lookups at the base level never mix two faces: every texel a lookup inside a chart
+    reads belongs to that chart's face.  Mipmaps a viewer builds do mix neighbouring charts at a distance, and texel density
+    varies up to about 2x between faces (each chart fills its power-of-two cell).  Raises ValueError when the mesh has more
+    faces than the texture holds (``ops.atlas_face_budget``)."""
+    aabb = [float(v) for v in nerf.aabb.tolist()]
+    geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
+    packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
+    return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size))
 
 
 _PLY_PROPS = {"vertices": ("x", "y", "z"), "normals": ("nx", "ny", "nz"), "colors": ("red", "green", "blue")}
@@ -104,6 +145,89 @@ def read_ply(path: str) -> dict:
     for k, ps in _PLY_PROPS.items():
         if ps[0] in names:
             out[k] = np.stack([vrec[p] for p in ps], 1).copy()
+    return out
+
+
+def obj_paths(path: str):
+    """(obj, mtl, png) paths of :func:`write_obj`: ``<stem>.obj``, ``<stem>.mtl``, ``<stem>_albedo.png``."""
+    import os
+    stem = os.path.splitext(path)[0]
+    return path, stem + ".mtl", stem + "_albedo.png"
+
+
+def _lines(fmt: str, a: np.ndarray) -> str:
+    return (fmt * a.shape[0]) % tuple(a.reshape(-1).tolist()) if a.shape[0] else ""
+
+
+def write_obj(path: str, mesh: dict) -> None:
+    """Wavefront OBJ of a textured mesh (a :func:`bake_texture` result): ``path`` with ``v`` (and ``vn`` when the mesh has
+    normals), three ``vt`` per face (face f's corners are vt 3f + 1 .. 3f + 3) and ``f v/vt[/vn]``; ``<stem>.mtl`` with one
+    material whose ``map_Kd`` is ``<stem>_albedo.png``, the texture (8-bit RGB).  Floats are written with 9 significant digits,
+    so fp32 values read back exactly."""
+    import os
+    import cv2
+    obj, mtl, png = obj_paths(path)
+    v = np.ascontiguousarray(_np(mesh["vertices"]), np.float32)
+    f = np.ascontiguousarray(_np(mesh["faces"]), np.int64).reshape(-1, 3)
+    uv = np.ascontiguousarray(_np(mesh["uv"]), np.float32).reshape(-1, 2)
+    tex = np.ascontiguousarray(_np(mesh["texture"]), np.uint8)
+    nrm = mesh.get("normals")
+    F = f.shape[0]
+    vi = f + 1
+    ti = np.arange(1, 3 * F + 1, dtype=np.int64).reshape(F, 3)
+    if nrm is not None:
+        idx, ffmt = np.stack([vi, ti, vi], 2), "f %d/%d/%d %d/%d/%d %d/%d/%d\n"
+    else:
+        idx, ffmt = np.stack([vi, ti], 2), "f %d/%d %d/%d %d/%d\n"
+    with open(obj, "w") as fh:
+        fh.write(f"# {v.shape[0]} vertices, {F} faces\nmtllib {os.path.basename(mtl)}\n")
+        fh.write(_lines("v %.9g %.9g %.9g\n", v.astype(np.float64)))
+        if nrm is not None:
+            fh.write(_lines("vn %.9g %.9g %.9g\n", np.ascontiguousarray(_np(nrm), np.float32).astype(np.float64)))
+        fh.write(_lines("vt %.9g %.9g\n", uv.astype(np.float64)))
+        fh.write("usemtl albedo\n")
+        fh.write(_lines(ffmt, idx.reshape(F, -1)))
+    with open(mtl, "w") as fh:
+        fh.write(f"newmtl albedo\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd {os.path.basename(png)}\n")
+    if not cv2.imwrite(png, np.ascontiguousarray(tex[:, :, ::-1])):
+        raise OSError(f"write_obj: could not write {png}")
+
+
+def read_obj(path: str) -> dict:
+    """Reads what :func:`write_obj` writes (numpy arrays): vertices, faces, uv [F,3,2], normals when present, and texture
+    [T,T,3] RGB from the PNG the MTL's ``map_Kd`` names."""
+    import os
+    import cv2
+    v, vn, vt, fl, mtl = [], [], [], [], None
+    with open(path) as fh:
+        for ln in fh:
+            w = ln.split()
+            if not w:
+                continue
+            if w[0] == "v":
+                v.append(w[1:4])
+            elif w[0] == "vn":
+                vn.append(w[1:4])
+            elif w[0] == "vt":
+                vt.append(w[1:3])
+            elif w[0] == "f":
+                fl.append([int(x) for c in w[1:4] for x in c.split("/")])
+            elif w[0] == "mtllib":
+                mtl = w[1]
+    per = len(fl[0]) // 3 if fl else 2
+    fa = np.asarray(fl, np.int64).reshape(-1, 3, per)
+    vt = np.asarray(vt, np.float32).reshape(-1, 2)
+    out = {"vertices": np.asarray(v, np.float32).reshape(-1, 3), "faces": (fa[:, :, 0] - 1).astype(np.int32),
+           "uv": vt[fa[:, :, 1] - 1] if len(fa) else np.zeros((0, 3, 2), np.float32)}
+    if vn:
+        out["normals"] = np.asarray(vn, np.float32).reshape(-1, 3)
+    if mtl is not None:
+        base = os.path.dirname(path)
+        with open(os.path.join(base, mtl)) as fh:
+            png = next(ln.split(None, 1)[1].strip() for ln in fh if ln.startswith("map_Kd"))
+        out["mtl"], out["map_Kd"] = mtl, png
+        img = cv2.imread(os.path.join(base, png), cv2.IMREAD_UNCHANGED)
+        out["texture"] = np.ascontiguousarray(img[:, :, ::-1])
     return out
 
 

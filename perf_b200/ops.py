@@ -773,6 +773,119 @@ def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, sta
     return pos, faces
 
 
+ATLAS_MIN_SIDE = 4          # smallest cell: two charts of leg 1 texel
+
+
+def atlas_face_budget(size: int) -> int:
+    """Most faces a ``size`` x ``size`` atlas holds: every face in the smallest class, two per 4 x 4 cell."""
+    return 2 * (size * size // (ATLAS_MIN_SIDE * ATLAS_MIN_SIDE))
+
+
+def _atlas_classes(legs: torch.Tensor, d: float, size: int):
+    """Face count per class, index 0 = side 4 (the last entry counts the faces that need a side above ``size``), for the
+    density ``d``: the class of a face is the smallest side s = 2^j >= 4 with fp32(leg * d) <= s - 3."""
+    bounds = torch.tensor([float((1 << j) - 3) for j in range(2, size.bit_length())], dtype=torch.float32, device=legs.device)
+    idx = torch.bucketize(legs * torch.tensor(d, dtype=torch.float32, device=legs.device), bounds)
+    return idx, [int(c) for c in torch.bincount(idx, minlength=len(bounds) + 1).tolist()]
+
+
+def _atlas_area(counts) -> int:
+    """Texels of the cells, or -1 when a face needs a class above the texture."""
+    if counts[-1]:
+        return -1
+    return sum((n + 1) // 2 * (1 << (2 * (j + 2))) for j, n in enumerate(counts[:-1]))
+
+
+def _f32_bits(b: int) -> float:
+    import struct
+    return struct.unpack("<f", struct.pack("<I", b))[0]
+
+
+def texture_atlas(vertices: torch.Tensor, faces: torch.Tensor, size: int) -> dict:
+    """Texture atlas of a triangle mesh (vertices [V,3] fp32, faces [F,3] int32) on a ``size`` x ``size`` texture (a power of
+    two in [256, 16384]): one right-isosceles chart per face, two faces per power-of-two cell, the cells packed along the
+    Z-order curve (``perf_atlas_legs`` / ``perf_atlas_layout``; include/perfb200.h states the rules).  The density d (texels per
+    world unit) is found by a bisection over the fp32 bit patterns: the size classes grow with it, and it ends at the largest d
+    of the last bracket where the cells still fit.  Returns {"uv": [F,3,2] fp32 (v up), "face_rec": [F,4] int32, "cells": [C,4]
+    int32, "density": d, "size": size, "used": texels the cells cover}; :func:`atlas_texels` takes it.  Raises ValueError when
+    the faces do not fit even in the smallest class (more than :func:`atlas_face_budget`)."""
+    if isinstance(size, bool) or int(size) != size or not (256 <= size <= 16384) or size & (size - 1):
+        raise ValueError(f"texture_atlas: size must be a power of two in [256, 16384], got {size!r}")
+    size = int(size)
+    if not isinstance(vertices, torch.Tensor) or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"texture_atlas: vertices must be [V, 3], got {getattr(vertices, 'shape', type(vertices))}")
+    if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"texture_atlas: faces must be [F, 3], got {getattr(faces, 'shape', type(faces))}")
+    budget = atlas_face_budget(size)
+    if faces.shape[0] > budget:
+        raise ValueError(f"texture_atlas: {faces.shape[0]} faces do not fit a {size}^2 texture, which holds at most {budget} "
+                         f"faces (two per {ATLAS_MIN_SIDE}x{ATLAS_MIN_SIDE} cell): decimate the mesh further (target_faces) "
+                         f"or use a larger texture size")
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
+    L = _L()
+    with torch.cuda.device(dev):
+        if F:
+            lo_i, hi_i = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
+            if lo_i < 0 or hi_i >= V:
+                raise ValueError(f"texture_atlas: face indices span [{lo_i}, {hi_i}], outside [0, {V})")
+        legs = torch.empty(F, dtype=torch.float32, device=dev)
+        _call(L.perf_atlas_legs, _p(vertices), V, _p(faces), F, _p(legs), _stream())
+        total = size * size
+        lo, hi = 0, 0x7F800000                          # fp32 bits: fits(lo) holds, hi = +inf is never tried
+        while hi - lo > 1:
+            mid = (lo + hi) // 2
+            a = _atlas_area(_atlas_classes(legs, _f32_bits(mid), size)[1])
+            if 0 <= a <= total:
+                lo = mid
+            else:
+                hi = mid
+        d = _f32_bits(lo)
+        idx, counts = _atlas_classes(legs, d, size)
+        order = torch.argsort(-idx, stable=True).to(torch.int32)
+        classes, pos, cell, off = [], 0, 0, 0
+        for j in range(len(counts) - 2, -1, -1):
+            n, s = counts[j], ATLAS_MIN_SIDE << j
+            if n:
+                classes.append((pos, n, cell, off, s))
+                pos, cell, off = pos + n, cell + (n + 1) // 2, off + (n + 1) // 2 * s * s
+        uv = torch.empty(F, 3, 2, dtype=torch.float32, device=dev)
+        rec = torch.empty(F, 4, dtype=torch.int32, device=dev)
+        cells = torch.empty(cell, 4, dtype=torch.int32, device=dev)
+        h = (C.c_int32 * max(1, 5 * len(classes)))(*[v for c in classes for v in c])
+        _call(L.perf_atlas_layout, _p(vertices), V, _p(faces), F, size, _p(order), h, len(classes), _p(uv), _p(rec), _p(cells), _stream())
+    return {"uv": uv, "face_rec": rec, "cells": cells, "density": d, "size": size, "used": off}
+
+
+def atlas_texels(vertices: torch.Tensor, faces: torch.Tensor, atlas: dict, m0: int = 0, n: Optional[int] = None):
+    """Texels m in [m0, m0 + n) (default: every texel the cells cover) of ``atlas`` (:func:`texture_atlas` of this mesh), in
+    Morton order: (face [n] int32, -1 where unused; point [n,3] fp32 world, the chart point nearest to the texel centre
+    mapped onto the face): ``perf_atlas_texels``."""
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    size = atlas["size"]
+    n = atlas["used"] - m0 if n is None else int(n)
+    if m0 < 0 or n < 0 or m0 + n > size * size:
+        raise ValueError(f"atlas_texels: range [{m0}, {m0 + n}) outside [0, {size * size})")
+    dev = vertices.device
+    face = torch.empty(n, dtype=torch.int32, device=dev)
+    point = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_atlas_texels, _p(vertices), vertices.shape[0], _p(faces), faces.shape[0], _p(atlas["face_rec"]),
+              _p(atlas["cells"]), atlas["cells"].shape[0], int(m0), n, _p(face), _p(point), _stream())
+    return face, point
+
+
+def morton_xy(m: torch.Tensor):
+    """(x, y) of Morton indices m (int64): x from the even bits, y from the odd bits."""
+    def compact(v):
+        v = v & 0x5555555555555555
+        for sh, mask in ((1, 0x3333333333333333), (2, 0x0F0F0F0F0F0F0F0F), (4, 0x00FF00FF00FF00FF), (8, 0x0000FFFF0000FFFF),
+                         (16, 0x00000000FFFFFFFF)):
+            v = (v | (v >> sh)) & mask
+        return v
+    return compact(m), compact(m >> 1)
+
+
 # ------------------------------------------------------------------ fused training step
 class FusedTrainContext:
     """Everything one fused training step needs besides the rays: the fp16 shadows / gather table,

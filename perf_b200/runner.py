@@ -205,21 +205,29 @@ class CoreRunner:
         to ``<exp_dir>/mesh/mesh_<res>.ply`` (binary PLY); extracted on the calling rank alone.  Like ``render_dense`` it uses
         the scene as constructed (``is_continue: true`` loads the checkpoint).  Config keys ``mesh_resolution`` (default 512)
         and ``mesh_threshold`` (default ``mesh.DEFAULT_THRESHOLD``); with ``mesh_target_faces`` the mesh is decimated to about
-        that many faces and written to ``mesh_<res>_f<target>.ply``, so a full mesh is never overwritten.  Returns (path, mesh)
-        on rank 0, else (None, None)."""
-        from .mesh import write_ply
+        that many faces and written to ``mesh_<res>_f<target>.ply``, so a full mesh is never overwritten.  With
+        ``mesh_texture_size`` the colour field is also baked into a texture atlas of that side and the textured mesh written
+        beside the PLY as ``<same stem>.obj`` / ``.mtl`` / ``_albedo.png`` (the PLY is the same either way).  Returns (path,
+        mesh) on rank 0, else (None, None)."""
+        from .mesh import write_obj, write_ply
         if not self.is_main:
             return None, None
         res = int(resolution if resolution is not None else self.conf.get("mesh_resolution", 512))
         thr = threshold if threshold is not None else self.conf.get("mesh_threshold", None)
         target = self.conf.get("mesh_target_faces", None)
         target = None if target is None else int(target)
+        tex = self.conf.get("mesh_texture_size", None)
         self.set_eval()
-        mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target)
+        if tex is None:
+            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target)
+        else:
+            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, texture_size=int(tex))
         os.makedirs(pjoin(self.exp_dir, "mesh"), exist_ok=True)
         name = "mesh_{}.ply".format(res) if target is None else "mesh_{}_f{}.ply".format(res, target)
         path = pjoin(self.exp_dir, "mesh", name)
         write_ply(path, mesh)
+        if tex is not None:
+            write_obj(path[:-len(".ply")] + ".obj", mesh)
         return path, mesh
 
     @staticmethod
