@@ -315,6 +315,54 @@ int perf_decimate_compact(const float* d_vertices, const double* d_quadrics, uin
                           const int32_t* d_faces, uint64_t F, const uint8_t* d_falive, const int32_t* d_foff,
                           float* d_out_vertices, double* d_out_quadrics, int32_t* d_out_faces, void* stream);
 
+/* ---- topological-noise removal for the decimation (opt-in: ops.decimate(max_cut=, min_component=); csrc/decimate.cu).  A
+ * briefly fitted field leaves small handles through its walls and floaters in free space; the link condition keeps both, so
+ * the collapse stalls.  Same input contract, half-edges and adjacency as the decimation above.
+ * Components: vertices are connected when a face holds both; label(v) = the smallest vertex index of v's component, a
+ *   face's label that of its vertex 0.  The label is unique, so any union-find gives it: hook (half-edge u -> w: atomicMin of
+ *   label[label[u]] with label[w] when that is smaller), then pointer-jump each vertex to its root; passes until neither
+ *   changes anything.  Box: per label, integer atomicMin/Max of the order-preserving int32 image of the fp32 coordinates
+ *   (b >= 0 ? b : b ^ 0x7FFFFFFF of the bits).  Diagonal^2 = (dx dx + dy dy) + dz dz in fp64, d = fp64(hi) - fp64(lo), one
+ *   rounded operation per step; a component is dropped iff diagonal^2 < min_component^2 (fp64).  Dropped vertices and faces
+ *   are cleared in valive / falive and perf_decimate_compact removes them (order kept, vertices renumbered ascending).
+ * Cut candidates: half-edge i = u -> w, u < w, link count > 2, opposite vertices o1 (of i) and o2 (of w -> u): the third
+ *   vertices x in N(u) n N(w) \ {o1, o2} with x > w, so a 3-cycle {a < b < c} is found once, from edge (a, b).  Perimeter p =
+ *   fp32((|u - w| + |w - x|) + |x - u|), |d| = sqrt((dx dx + dy dy) + dz dz), fp64 with rounded steps.  The candidate is the x
+ *   of smallest (p, x) with p <= max_cut (fp32) and u, w, x vertex-manifold (the fan walk below from a vertex's first corner
+ *   visits all its corners); key = fp32 bits(p) << 32 | i, INT64_MAX when there is none.
+ * Selection: m1[v] = min key over the candidates at v in {u, w, x}; m2[v] = min of m1 over v and N(v); cycle selected iff
+ *   key == m2[u] == m2[w] == m2[x].  Two selected cycles s, t (key_s < key_t) share no vertex and no edge between their
+ *   vertices: a vertex b of t equal or adjacent to a vertex of s would have m2[b] <= key_s < key_t.  So their fans are
+ *   disjoint and the cuts run in parallel without races.
+ * Cut of selected cycle s (s-th in ascending half-edge order), u -> w -> x: fan step at v from corner c = v's corner whose
+ *   next is c's prev.  The left arc of cycle vertex v runs from the face of its outgoing cycle half-edge (v's next is the
+ *   next cycle vertex) by fan steps to, and including, the face of its incoming one (v's prev is the previous cycle vertex).
+ *   New vertices u', w', x' at V + 3s + {0, 1, 2} copy position and quadric; v becomes v' in exactly its left arc's corners;
+ *   all three arcs are walked before any corner is rewritten.  Caps (u, w, x) and (u', x', w') at F + 2s and F + 2s + 1 (no
+ *   quadric).  Every directed edge still appears once with its opposite; the genus drops by 1 or the component count rises
+ *   by 1: chi rises by 2.
+ * Driver (ops.decimate): with min_component, drop before the first round; collapse rounds as above (bit-identical to a call
+ *   without the new arguments up to the first stall when nothing is dropped); when a round selects nothing, F > target and
+ *   max_cut is set: one cut round, the component drop, collapse rounds again; stop when F <= target or a cut round selects
+ *   nothing. */
+/* One union-find pass: hook over the half-edges, pointer jump over the vertices (two launches).  d_label [V] int32 = 0 .. V - 1
+ * before the first pass; d_changed [1] int32, zeroed by the caller, becomes nonzero when the pass changed a label. */
+int perf_decimate_components(const int32_t* d_faces, uint64_t F, uint64_t V, int32_t* d_label, int32_t* d_changed, void* stream);
+/* d_box [V,6] int32 per label (min xyz, max xyz images), set by the caller to INT32_MAX x 3, INT32_MIN x 3; d_valive [V] /
+ * d_falive [F] uint8 = 1 unless dropped (three launches). */
+int perf_decimate_component_box(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_label,
+                                double min_component, int32_t* d_box, uint8_t* d_valive, uint8_t* d_falive, void* stream);
+/* Per half-edge: d_key [3F] int64, d_third [3F] int32 (x, candidates only); d_vmin [V] = m1 (caller-set INT64_MAX). */
+int perf_decimate_cycles(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_adj,
+                         const int32_t* d_adj_off, float max_cut, int64_t* d_key, int32_t* d_third, int64_t* d_vmin, void* stream);
+/* d_vmin2 [V] = m2 (the caller copies m1 into it), d_selected [3F] uint8 (two launches). */
+int perf_decimate_cycle_select(const int32_t* d_faces, uint64_t F, uint64_t V, const int64_t* d_key, const int32_t* d_third,
+                               const int64_t* d_vmin, int64_t* d_vmin2, uint8_t* d_selected, void* stream);
+/* Cuts the n selected cycles d_cycles (half-edge ids, ascending) in place: d_vertices [V + 3n, 3] and d_quadrics [V + 3n, 10]
+ * hold the mesh's V rows first, d_faces [F + 2n, 3] its F faces; d_adj / d_adj_off are the F-face mesh's. */
+int perf_decimate_cut(const int64_t* d_cycles, uint64_t n, const int32_t* d_third, float* d_vertices, double* d_quadrics, uint64_t V,
+                      int32_t* d_faces, uint64_t F, const int32_t* d_adj, const int32_t* d_adj_off, void* stream);
+
 /* ---- texture atlas of a triangle mesh (ops.texture_atlas drives it; csrc/texture.cu).  A T x T texture, T a power of two in
  * [256, 16384]; texel (x, y) (y up: image row T - 1 - y) covers [x, x + 1] x [y, y + 1] in texel units and has the Morton
  * index m = interleave(x in the even bits, y in the odd bits).

@@ -94,6 +94,11 @@ SIGNATURES = {
     "perf_decimate_select": (i32, [vp, u64, u64, vp, vp, vp, vp, vp]),
     "perf_decimate_collapse": (i32, [vp, u64, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]),
     "perf_decimate_compact": (i32, [vp, vp, u64, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_decimate_components": (i32, [vp, u64, u64, vp, vp, vp]),
+    "perf_decimate_component_box": (i32, [vp, u64, vp, u64, vp, C.c_double, vp, vp, vp, vp]),
+    "perf_decimate_cycles": (i32, [vp, u64, vp, u64, vp, vp, f32, vp, vp, vp, vp]),
+    "perf_decimate_cycle_select": (i32, [vp, u64, u64, vp, vp, vp, vp, vp, vp]),
+    "perf_decimate_cut": (i32, [vp, u64, vp, vp, vp, u64, vp, u64, vp, vp, vp]),
     "perf_atlas_legs": (i32, [vp, u64, vp, u64, vp, vp]),
     "perf_atlas_layout": (i32, [vp, u64, vp, u64, i32, vp, P(i32), i32, vp, vp, vp, vp]),
     "perf_atlas_texels": (i32, [vp, u64, vp, u64, vp, vp, u64, u64, u64, vp, vp, vp]),

@@ -29,7 +29,8 @@ namespace perf {
 constexpr int64_t DEC_NO_KEY = 0x7FFFFFFFFFFFFFFFll;   // no candidate edge (above every key: cost bits < 2^31)
 constexpr double DEC_COND = 1e-6;                      // det(A) > DEC_COND * trace(A)^3: the 3x3 system is solved
 
-enum { DEC_CHECK, DEC_QUADRICS, DEC_EDGES, DEC_VMIN2, DEC_SELECT, DEC_COLLAPSE, DEC_COMPACT_F, DEC_COMPACT_V };
+enum { DEC_CHECK, DEC_QUADRICS, DEC_EDGES, DEC_VMIN2, DEC_SELECT, DEC_COLLAPSE, DEC_COMPACT_F, DEC_COMPACT_V,
+       DEC_HOOK, DEC_JUMP, DEC_BOX, DEC_DROP_V, DEC_DROP_F, DEC_CYCLES, DEC_CYCLE_SELECT, DEC_CUT };
 
 struct DecArgs {
     float* pos; double* quad; int64_t V;                  // [V,3] fp32, [V,10] fp64
@@ -42,6 +43,12 @@ struct DecArgs {
     const int32_t* voff; const int32_t* foff;             // exclusive scans of valive / falive
     float* out_pos; double* out_quad; int32_t* out_faces;
     int32_t* flags;
+};
+
+// The topological-noise removal stages: the collapse fields plus their own (a separate kernel, so DecArgs keeps its size).
+struct DecCleanArgs : DecArgs {
+    int32_t* label; int32_t* box; double min_comp;        // component label [V], box [V,6] int32 images, drop diagonal
+    int32_t* third; float max_cut;                        // cycle's third vertex [3F], longest perimeter cut
 };
 
 struct D3 { double x, y, z; };
@@ -258,6 +265,180 @@ __host__ __device__ __forceinline__ void dec_compact_vertex(const DecArgs& a, in
     for (int t = 0; t < 10; ++t) a.out_quad[10 * o + t] = a.quad[10 * v + t];
 }
 
+// ---- topological-noise removal: components, their boxes and the drop; short non-face 3-cycles and the cut along them.
+
+__host__ __device__ __forceinline__ void dec_flag(int32_t* p)
+{
+#ifdef __CUDA_ARCH__
+    atomicOr((int*)p, 1);
+#else
+    *p |= 1;
+#endif
+}
+
+// Hook, half-edge u -> w: the label of u's label drops to w's when that is smaller (a forest whose parents are smaller).
+__host__ __device__ __forceinline__ void dec_hook(const DecCleanArgs& a, int64_t i)
+{
+    const int32_t lu = a.label[a.faces[i]], lw = a.label[dec_next(a, i)];
+    if (!(lw < lu)) return;
+#ifdef __CUDA_ARCH__
+    atomicMin((int*)&a.label[lu], (int)lw);
+#else
+    if (lw < a.label[lu]) a.label[lu] = lw;
+#endif
+    dec_flag(a.flags);
+}
+
+// Pointer jump of vertex v to its root.  Other threads only lower labels to ancestors, so any value read is an ancestor.
+__host__ __device__ __forceinline__ void dec_jump(const DecCleanArgs& a, int64_t v)
+{
+    volatile int32_t* lab = a.label;
+    int32_t l = lab[v], n;
+    while ((n = lab[l]) != l) l = n;
+    if (l != lab[v]) { lab[v] = l; dec_flag(a.flags); }
+}
+
+// Order-preserving int32 image of an fp32 value (and its inverse: the same map).
+__host__ __device__ __forceinline__ int32_t dec_ord(int32_t b) { return b >= 0 ? b : b ^ 0x7FFFFFFF; }
+
+__host__ __device__ __forceinline__ void dec_box(const DecCleanArgs& a, int64_t v)
+{
+    const int64_t l = a.label[v];
+    for (int d = 0; d < 3; ++d) {
+        int32_t b;
+        memcpy(&b, &a.pos[3 * v + d], sizeof(b));
+        b = dec_ord(b);
+#ifdef __CUDA_ARCH__
+        atomicMin((int*)&a.box[6 * l + d], (int)b);
+        atomicMax((int*)&a.box[6 * l + 3 + d], (int)b);
+#else
+        if (b < a.box[6 * l + d]) a.box[6 * l + d] = b;
+        if (b > a.box[6 * l + 3 + d]) a.box[6 * l + 3 + d] = b;
+#endif
+    }
+}
+
+// Vertex v survives iff the diagonal^2 of its component's box, (dx^2 + dy^2) + dz^2 in fp64, is not below min_comp^2.
+__host__ __device__ __forceinline__ void dec_drop_vertex(const DecCleanArgs& a, int64_t v)
+{
+    const int64_t l = a.label[v];
+    double e[3];
+    for (int d = 0; d < 3; ++d) {
+        const int32_t lo = dec_ord(a.box[6 * l + d]), hi = dec_ord(a.box[6 * l + 3 + d]);
+        float flo, fhi;
+        memcpy(&flo, &lo, sizeof(flo));
+        memcpy(&fhi, &hi, sizeof(fhi));
+        e[d] = PERF_DSUB_RN((double)fhi, (double)flo);
+    }
+    const double d2 = PERF_DADD_RN(PERF_DADD_RN(PERF_DMUL_RN(e[0], e[0]), PERF_DMUL_RN(e[1], e[1])), PERF_DMUL_RN(e[2], e[2]));
+    a.valive[v] = !(d2 < PERF_DMUL_RN(a.min_comp, a.min_comp));
+}
+
+__host__ __device__ __forceinline__ void dec_drop_face(const DecCleanArgs& a, int64_t f) { a.falive[f] = a.valive[a.faces[3 * f]]; }
+
+// Fan step around v from corner c: v's corner whose next is c's prev (-1 if none).
+__host__ __device__ __forceinline__ int32_t dec_fan_step(const DecArgs& a, int32_t v, int32_t c)
+{
+    const int32_t p = dec_prev(a, c);
+    for (int32_t t = a.adj_off[v]; t < a.adj_off[v + 1]; ++t) if (dec_next(a, a.adj[t]) == p) return a.adj[t];
+    return -1;
+}
+
+// v is vertex-manifold iff the fan walk from its first corner visits all its corners before it returns.
+__host__ __device__ __forceinline__ bool dec_manifold(const DecArgs& a, int32_t v)
+{
+    const int32_t n = dec_valence(a, v), c0 = a.adj[a.adj_off[v]];
+    int32_t c = c0, k = 0;
+    do { c = dec_fan_step(a, v, c); ++k; } while (c >= 0 && c != c0 && k <= n);
+    return c == c0 && k == n;
+}
+
+__host__ __device__ __forceinline__ double dec_len(D3 p, D3 q) { const D3 d = dec_sub(p, q); return PERF_DSQRT_RN(dec_dot(d, d)); }
+
+// Half-edge i from u to w, u < w, link count > 2: the non-face 3-cycle u -> w -> x (x > w, not an opposite vertex, u w x
+// vertex-manifold) of smallest (perimeter, x) with perimeter <= max_cut; key, third vertex, m1 over u, w, x.
+__host__ __device__ __forceinline__ void dec_cycles(const DecCleanArgs& a, int64_t i)
+{
+    a.key[i] = DEC_NO_KEY;
+    const int32_t u = a.faces[i], w = dec_next(a, i);
+    if (!(u < w)) return;
+    int32_t o2 = -1, link = 0;
+    for (int32_t c = a.adj_off[w]; c < a.adj_off[w + 1]; ++c) if (dec_next(a, a.adj[c]) == u) o2 = dec_prev(a, a.adj[c]);
+    for (int32_t c = a.adj_off[u]; c < a.adj_off[u + 1]; ++c) {
+        const int32_t x = dec_next(a, a.adj[c]);
+        for (int32_t c2 = a.adj_off[w]; c2 < a.adj_off[w + 1]; ++c2)
+            if (dec_next(a, a.adj[c2]) == x) { ++link; break; }
+    }
+    if (link <= 2 || !dec_manifold(a, u) || !dec_manifold(a, w)) return;
+    const int32_t o1 = dec_prev(a, i);
+    const D3 pu = dec_pos(a.pos, u), pw = dec_pos(a.pos, w);
+    const double luw = dec_len(pu, pw);
+    float best = 0.0f;
+    int32_t bx = -1;
+    for (int32_t c = a.adj_off[u]; c < a.adj_off[u + 1]; ++c) {
+        const int32_t x = dec_next(a, a.adj[c]);
+        if (x <= w || x == o1 || x == o2) continue;
+        bool in_w = false;
+        for (int32_t c2 = a.adj_off[w]; c2 < a.adj_off[w + 1]; ++c2) in_w |= dec_next(a, a.adj[c2]) == x;
+        if (!in_w) continue;
+        const D3 px = dec_pos(a.pos, x);
+        const float p = PERF_D2F_RN(PERF_DADD_RN(PERF_DADD_RN(luw, dec_len(pw, px)), dec_len(px, pu)));
+        if (!(p <= a.max_cut) || (bx >= 0 && (p > best || (p == best && x > bx))) || !dec_manifold(a, x)) continue;
+        best = p; bx = x;
+    }
+    if (bx < 0) return;
+    uint32_t bits;
+    memcpy(&bits, &best, sizeof(bits));
+    const int64_t k = (int64_t)((uint64_t)bits << 32 | (uint64_t)i);
+    a.key[i] = k;
+    a.third[i] = bx;
+    dec_min(&a.vmin[u], k);
+    dec_min(&a.vmin[w], k);
+    dec_min(&a.vmin[bx], k);
+}
+
+__host__ __device__ __forceinline__ void dec_cycle_select(const DecCleanArgs& a, int64_t i)
+{
+    const int64_t k = a.key[i];
+    a.sel[i] = k != DEC_NO_KEY && a.vmin2[a.faces[i]] == k && a.vmin2[dec_next(a, i)] == k && a.vmin2[a.third[i]] == k;
+}
+
+// Cut along selected cycle s (half-edge e = edges[s], u -> w -> x): in each cycle vertex's left arc (from the face of its
+// outgoing cycle half-edge, stepping around the fan, to the face of its incoming one) the vertex becomes its copy at
+// V + 3s + j; caps (u, w, x) and (u', x', w') at F + 2s.  All three arcs are walked before any corner is rewritten: the face
+// of u -> w ends w's arc, and rewriting u there first would hide it.  The arcs' interior spokes are not cycle vertices, so
+// the second walk of each arc, by its length, is not disturbed by the other arcs' rewrites.
+__host__ __device__ __forceinline__ void dec_cut(const DecCleanArgs& a, int64_t s)
+{
+    const int64_t e = a.edges[s];
+    const int32_t cyc[3] = {a.faces[e], dec_next(a, e), a.third[e]};
+    int32_t start[3], len[3];
+    for (int j = 0; j < 3; ++j) {
+        const int32_t v = cyc[j], n = cyc[(j + 1) % 3], p = cyc[(j + 2) % 3];
+        int32_t c = -1;
+        for (int32_t t = a.adj_off[v]; t < a.adj_off[v + 1]; ++t) if (dec_next(a, a.adj[t]) == n) c = a.adj[t];
+        start[j] = c;
+        int32_t k = 1;
+        while (dec_prev(a, c) != p) { c = dec_fan_step(a, v, c); ++k; }
+        len[j] = k;
+    }
+    for (int j = 0; j < 3; ++j) {
+        const int32_t v = cyc[j], vn = (int32_t)(a.V + 3 * s + j);
+        int32_t c = start[j];
+        for (int32_t k = 0; k < len[j]; ++k) {
+            const int32_t next = k + 1 < len[j] ? dec_fan_step(a, v, c) : -1;
+            a.faces[c] = vn;
+            c = next;
+        }
+        for (int d = 0; d < 3; ++d) a.pos[3 * (int64_t)vn + d] = a.pos[3 * (int64_t)v + d];
+        for (int t = 0; t < 10; ++t) a.quad[10 * (int64_t)vn + t] = a.quad[10 * (int64_t)v + t];
+    }
+    int32_t* cap = a.faces + 3 * (a.F + 2 * s);
+    const int32_t b = (int32_t)(a.V + 3 * s);
+    cap[0] = cyc[0]; cap[1] = cyc[1]; cap[2] = cyc[2];
+    cap[3] = b; cap[4] = b + 2; cap[5] = b + 1;
+}
+
 template <int S>
 __host__ __device__ __forceinline__ void dec_body(const DecArgs& a, int64_t i)
 {
@@ -272,10 +453,30 @@ __host__ __device__ __forceinline__ void dec_body(const DecArgs& a, int64_t i)
 }
 
 template <int S>
+__host__ __device__ __forceinline__ void dec_clean_body(const DecCleanArgs& a, int64_t i)
+{
+    if (S == DEC_HOOK) dec_hook(a, i);
+    else if (S == DEC_JUMP) dec_jump(a, i);
+    else if (S == DEC_BOX) dec_box(a, i);
+    else if (S == DEC_DROP_V) dec_drop_vertex(a, i);
+    else if (S == DEC_DROP_F) dec_drop_face(a, i);
+    else if (S == DEC_CYCLES) dec_cycles(a, i);
+    else if (S == DEC_CYCLE_SELECT) dec_cycle_select(a, i);
+    else dec_cut(a, i);
+}
+
+template <int S>
 __global__ void __launch_bounds__(128) decimate_kernel(const DecArgs a, int64_t n)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) dec_body<S>(a, i);
+}
+
+template <int S>
+__global__ void __launch_bounds__(128) decimate_clean_kernel(const DecCleanArgs a, int64_t n)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dec_clean_body<S>(a, i);
 }
 
 // The product library launches the kernel; the test harness build runs the same body over host arrays.
@@ -288,6 +489,20 @@ static int dec_run(const DecArgs& a, int64_t n, void* stream)
     for (int64_t i = 0; i < n; ++i) dec_body<S>(a, i);
 #else
     decimate_kernel<S><<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a, n);
+    PERF_LAUNCH_CHECK();
+#endif
+    return PERF_OK;
+}
+
+template <int S>
+static int dec_run(const DecCleanArgs& a, int64_t n, void* stream)
+{
+    if (n <= 0) return PERF_OK;
+#ifdef PERF_HOST_HARNESS
+    (void)stream;
+    for (int64_t i = 0; i < n; ++i) dec_clean_body<S>(a, i);
+#else
+    decimate_clean_kernel<S><<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a, n);
     PERF_LAUNCH_CHECK();
 #endif
     return PERF_OK;
@@ -378,6 +593,70 @@ int perf_decimate_compact(const float* d_vertices, const double* d_quadrics, uin
     a.out_pos = d_out_vertices; a.out_quad = d_out_quadrics; a.out_faces = d_out_faces;
     int rc = dec_run<DEC_COMPACT_F>(a, (int64_t)F, stream); if (rc) return rc;
     return dec_run<DEC_COMPACT_V>(a, (int64_t)V, stream);
+}
+
+int perf_decimate_components(const int32_t* d_faces, uint64_t F, uint64_t V, int32_t* d_label, int32_t* d_changed, void* stream)
+{
+    DecCleanArgs a;
+    PERF_CHECK_ARG(V < (1ull << 31) && 3 * F < (1ull << 31), "mesh too large");
+    PERF_CHECK_ARG(V == 0 || (d_label && d_changed && (F == 0 || d_faces)), "NULL pointer");
+    memset(&a, 0, sizeof(a));
+    a.V = (int64_t)V; a.F = (int64_t)F; a.faces = (int32_t*)d_faces; a.label = d_label; a.flags = d_changed;
+    int rc = dec_run<DEC_HOOK>(a, 3 * (int64_t)F, stream); if (rc) return rc;
+    return dec_run<DEC_JUMP>(a, (int64_t)V, stream);
+}
+
+int perf_decimate_component_box(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_label,
+                                double min_component, int32_t* d_box, uint8_t* d_valive, uint8_t* d_falive, void* stream)
+{
+    DecCleanArgs a;
+    PERF_CHECK_ARG(V < (1ull << 31) && 3 * F < (1ull << 31), "mesh too large");
+    PERF_CHECK_ARG(V == 0 || (d_vertices && d_label && d_box && d_valive), "NULL vertex array");
+    PERF_CHECK_ARG(F == 0 || (d_faces && d_falive), "NULL face array");
+    PERF_CHECK_ARG(min_component >= 0.0, "min_component %g < 0", min_component);
+    memset(&a, 0, sizeof(a));
+    a.pos = (float*)d_vertices; a.V = (int64_t)V; a.faces = (int32_t*)d_faces; a.F = (int64_t)F; a.label = (int32_t*)d_label;
+    a.min_comp = min_component; a.box = d_box; a.valive = d_valive; a.falive = d_falive;
+    int rc = dec_run<DEC_BOX>(a, (int64_t)V, stream); if (rc) return rc;
+    rc = dec_run<DEC_DROP_V>(a, (int64_t)V, stream); if (rc) return rc;
+    return dec_run<DEC_DROP_F>(a, (int64_t)F, stream);
+}
+
+int perf_decimate_cycles(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_adj,
+                         const int32_t* d_adj_off, float max_cut, int64_t* d_key, int32_t* d_third, int64_t* d_vmin, void* stream)
+{
+    DecCleanArgs a;
+    memset(&a, 0, sizeof(a));
+    int rc = dec_fill(a, V, d_faces, F, d_adj, d_adj_off); if (rc) return rc;
+    PERF_CHECK_ARG(F == 0 || (d_vertices && d_key && d_third && d_vmin), "NULL pointer");
+    a.pos = (float*)d_vertices; a.max_cut = max_cut; a.key = d_key; a.third = d_third; a.vmin = d_vmin;
+    return dec_run<DEC_CYCLES>(a, 3 * (int64_t)F, stream);
+}
+
+int perf_decimate_cycle_select(const int32_t* d_faces, uint64_t F, uint64_t V, const int64_t* d_key, const int32_t* d_third,
+                               const int64_t* d_vmin, int64_t* d_vmin2, uint8_t* d_selected, void* stream)
+{
+    DecCleanArgs a;
+    PERF_CHECK_ARG(V < (1ull << 31) && 3 * F < (1ull << 31), "mesh too large");
+    PERF_CHECK_ARG(F == 0 || (d_faces && d_key && d_third && d_vmin && d_vmin2 && d_selected), "NULL pointer");
+    memset(&a, 0, sizeof(a));
+    a.V = (int64_t)V; a.F = (int64_t)F; a.faces = (int32_t*)d_faces;
+    a.key = (int64_t*)d_key; a.third = (int32_t*)d_third; a.vmin = (int64_t*)d_vmin; a.vmin2 = d_vmin2; a.sel = d_selected;
+    int rc = dec_run<DEC_VMIN2>(static_cast<const DecArgs&>(a), 3 * (int64_t)F, stream); if (rc) return rc;
+    return dec_run<DEC_CYCLE_SELECT>(a, 3 * (int64_t)F, stream);
+}
+
+int perf_decimate_cut(const int64_t* d_cycles, uint64_t n, const int32_t* d_third, float* d_vertices, double* d_quadrics, uint64_t V,
+                      int32_t* d_faces, uint64_t F, const int32_t* d_adj, const int32_t* d_adj_off, void* stream)
+{
+    DecCleanArgs a;
+    memset(&a, 0, sizeof(a));
+    int rc = dec_fill(a, V, d_faces, F, d_adj, d_adj_off); if (rc) return rc;
+    PERF_CHECK_ARG(V + 3 * n < (1ull << 31) && 3 * (F + 2 * n) < (1ull << 31), "%llu cuts: the mesh outgrows int32 indices",
+                   (unsigned long long)n);
+    PERF_CHECK_ARG(n == 0 || (d_cycles && d_third && d_vertices && d_quadrics), "NULL pointer");
+    a.edges = d_cycles; a.n_edges = (int64_t)n; a.third = (int32_t*)d_third; a.pos = d_vertices; a.quad = d_quadrics;
+    return dec_run<DEC_CUT>(a, (int64_t)n, stream);
 }
 
 #pragma GCC visibility pop

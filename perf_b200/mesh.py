@@ -24,7 +24,8 @@ DEFAULT_THRESHOLD = 50.0
 
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
-                 normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None) -> dict:
+                 normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None,
+                 min_component: Optional[float] = None, max_cut: Optional[float] = None) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -33,14 +34,29 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     With ``target_faces`` the mesh is first decimated to about that many faces (``ops.decimate``: quadric-error edge
     collapse, which removes faces where the surface is flat and keeps them where it bends); colours and normals are then the
     fields' at the decimated vertices.  With ``texture_size`` the colour field is then baked into a texture atlas of that side
-    (:func:`bake_texture`): ``"uv"`` [F,3,2] and ``"texture"`` [T,T,3] uint8 join the dict."""
+    (:func:`bake_texture`): ``"uv"`` [F,3,2] and ``"texture"`` [T,T,3] uint8 join the dict.
+    ``min_component`` and ``max_cut`` remove a fit's topological noise, both in voxels of the lattice (the smallest of
+    extent / (r - 1) over the axes): components whose bounding-box diagonal is below ``min_component`` are dropped (floaters),
+    and with ``target_faces`` the decimation cuts the mesh along non-face 3-cycles of perimeter <= ``max_cut`` where it would
+    otherwise stall (short handles through the walls); ``ops.decimate`` states both.  ``max_cut`` needs ``target_faces``."""
+    if max_cut is not None and target_faces is None:
+        raise ValueError("extract_mesh: max_cut acts on the decimation: it needs target_faces")
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     sigma = ops.fields_lattice(packed, geo_half, app_half, resolution, aabb, PERF_GRID)
     verts, faces = ops.marching_tets(sigma, threshold, aabb)
     del sigma
-    if target_faces is not None:
+    if min_component is not None or max_cut is not None:
+        r3 = [int(resolution)] * 3 if isinstance(resolution, int) else [int(r) for r in resolution]
+        voxel = min((aabb[3 + d] - aabb[d]) / (r3[d] - 1) for d in range(3))
+        mc = None if min_component is None else float(min_component) * voxel
+        cut = None if max_cut is None else float(max_cut) * voxel
+        if target_faces is not None:
+            verts, faces = ops.decimate(verts, faces, target_faces, max_cut=cut, min_component=mc)
+        else:
+            verts, faces = ops.drop_components(verts, faces, mc)
+    elif target_faces is not None:
         verts, faces = ops.decimate(verts, faces, target_faces)
     out = {"vertices": verts, "faces": faces}
     if colors or normals:

@@ -7,6 +7,7 @@ CPU path: a non-CUDA tensor raises.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Optional
 
@@ -701,42 +702,159 @@ def _exclusive(flags: torch.Tensor) -> torch.Tensor:
     return torch.cumsum(flags, 0, dtype=torch.int32) - flags
 
 
-def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, stats: Optional[list] = None):
+def _check_length(name: str, value):
+    if value is None:
+        return None
+    if isinstance(value, bool) or not isinstance(value, (int, float)) or not math.isfinite(value) or value < 0:
+        raise ValueError(f"{name} must be a finite number >= 0 or None, got {value!r}")
+    return float(value)
+
+
+def _components(faces: torch.Tensor, V: int) -> torch.Tensor:
+    """Per vertex, the smallest vertex index of its component (``perf_decimate_components`` passes until nothing changes;
+    one host read per pass)."""
+    label = torch.arange(V, dtype=torch.int32, device=faces.device)
+    changed = torch.zeros(1, dtype=torch.int32, device=faces.device)
+    while True:
+        changed.zero_()
+        _call(_L().perf_decimate_components, _p(faces), faces.shape[0], V, _p(label), _p(changed), _stream(), launches=2)
+        if not int(changed.item()):
+            return label
+
+
+def _drop_components(pos, quad, faces, min_component: float):
+    """Drops the components whose box diagonal is below ``min_component`` (``perf_decimate_component_box``, then
+    ``perf_decimate_compact``) -> (pos, quad, faces, number of components dropped)."""
+    V, F, dev = pos.shape[0], faces.shape[0], pos.device
+    label = _components(faces, V)
+    box = torch.empty(V, 6, dtype=torch.int32, device=dev)
+    box[:, :3], box[:, 3:] = 2 ** 31 - 1, -2 ** 31
+    valive = torch.empty(V, dtype=torch.uint8, device=dev)
+    falive = torch.empty(F, dtype=torch.uint8, device=dev)
+    _call(_L().perf_decimate_component_box, _p(pos), V, _p(faces), F, _p(label), float(min_component), _p(box), _p(valive), _p(falive),
+          _stream(), launches=3)
+    roots = label == torch.arange(V, dtype=torch.int32, device=dev)
+    V2, F2, dropped = (int(v) for v in torch.stack([valive.sum(dtype=torch.int64), falive.sum(dtype=torch.int64),
+                                                    (roots & (valive == 0)).sum()]).tolist())
+    if dropped == 0:
+        return pos, quad, faces, 0
+    pos2 = torch.empty(V2, 3, dtype=torch.float32, device=dev)
+    quad2 = torch.empty(V2, 10, dtype=torch.float64, device=dev)
+    faces2 = torch.empty(F2, 3, dtype=torch.int32, device=dev)
+    voff, foff = _exclusive(valive), _exclusive(falive)
+    _call(_L().perf_decimate_compact, _p(pos), _p(quad), V, _p(valive), _p(voff), _p(faces), F, _p(falive), _p(foff),
+          _p(pos2), _p(quad2), _p(faces2), _stream(), launches=2)
+    return pos2, quad2, faces2, dropped
+
+
+def _cut_round(pos, quad, faces, adj, off, max_cut: float):
+    """One cut round (``perf_decimate_cycles`` / ``_cycle_select`` / ``_cut``) -> (pos, quad, faces, number of cuts)."""
+    L, V, F, dev = _L(), pos.shape[0], faces.shape[0], pos.device
+    key = torch.empty(3 * F, dtype=torch.int64, device=dev)
+    third = torch.empty(3 * F, dtype=torch.int32, device=dev)
+    vmin = torch.full((V,), _NO_KEY, dtype=torch.int64, device=dev)
+    _call(L.perf_decimate_cycles, _p(pos), V, _p(faces), F, _p(adj), _p(off), float(max_cut), _p(key), _p(third), _p(vmin), _stream())
+    vmin2, sel = vmin.clone(), torch.empty(3 * F, dtype=torch.uint8, device=dev)
+    _call(L.perf_decimate_cycle_select, _p(faces), F, V, _p(key), _p(third), _p(vmin), _p(vmin2), _p(sel), _stream(), launches=2)
+    cycles = torch.nonzero(sel).view(-1)                                     # ascending: the cut order
+    n = cycles.numel()
+    if n == 0:
+        return pos, quad, faces, 0
+    pos2 = torch.cat([pos, torch.empty(3 * n, 3, dtype=torch.float32, device=dev)])
+    quad2 = torch.cat([quad, torch.empty(3 * n, 10, dtype=torch.float64, device=dev)])
+    faces2 = torch.cat([faces, torch.empty(2 * n, 3, dtype=torch.int32, device=dev)])
+    _call(L.perf_decimate_cut, _p(cycles), n, _p(third), _p(pos2), _p(quad2), V, _p(faces2), F, _p(adj), _p(off), _stream())
+    return pos2, quad2, faces2, n
+
+
+def _check_shapes(name: str, vertices, faces):
+    if not isinstance(vertices, torch.Tensor) or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"{name}: vertices must be [V, 3], got {getattr(vertices, 'shape', type(vertices))}")
+    if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{name}: faces must be [F, 3], got {getattr(faces, 'shape', type(faces))}")
+
+
+def _prepare(name: str, vertices, faces):
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    V, F = vertices.shape[0], faces.shape[0]
+    if V >= 2 ** 31 or 3 * F >= 2 ** 31:
+        raise ValueError(f"{name}: {V} vertices / {F} faces: needs V < 2^31 and 3F < 2^31")
+    return vertices, faces
+
+
+def _check_closed(name: str, faces: torch.Tensor, V: int):
+    """Index range and ``perf_decimate_check`` -> the corner adjacency."""
+    F, dev = faces.shape[0], faces.device
+    lo, hi = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
+    if lo < 0 or hi >= V:
+        raise ValueError(f"{name}: face indices span [{lo}, {hi}], outside [0, {V})")
+    adj, off = _corner_adjacency(faces, V)
+    flags = torch.zeros(1, dtype=torch.int32, device=dev)
+    _call(_L().perf_decimate_check, _p(faces), F, V, _p(adj), _p(off), _p(flags), _stream())
+    bad = int(flags.item())
+    if bad:
+        raise ValueError(f"{name}: not a closed, consistently oriented, edge-manifold mesh: "
+                         + "; ".join(m for b, m in _DECIMATE_FLAGS.items() if bad & b))
+    return adj, off
+
+
+def drop_components(vertices: torch.Tensor, faces: torch.Tensor, min_component: float):
+    """Removes the connected components of a closed, consistently oriented, edge-manifold mesh whose axis-aligned bounding
+    box has a diagonal below ``min_component`` (world units): the floaters of a fitted field.  The kept faces and vertices
+    keep their order (vertices renumbered ascending).  Returns (vertices [V',3], faces [F',3]); include/perfb200.h states
+    the rule."""
+    _check_shapes("drop_components", vertices, faces)
+    mc = _check_length("min_component", min_component)
+    if mc is None:
+        raise ValueError("drop_components: min_component is required")
+    vertices, faces = _prepare("drop_components", vertices, faces)
+    V, dev = vertices.shape[0], vertices.device
+    if faces.shape[0] == 0:
+        return vertices.clone(), faces.clone()
+    with torch.cuda.device(dev):
+        _check_closed("drop_components", faces, V)
+        quad = torch.zeros(V, 10, dtype=torch.float64, device=dev)      # carried through the compaction, then discarded
+        pos, _, out, n = _drop_components(vertices, quad, faces, mc)
+    return (pos, out) if n else (vertices.clone(), faces.clone())
+
+
+def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, stats: Optional[list] = None,
+             max_cut: Optional[float] = None, min_component: Optional[float] = None):
     """Quadric-error edge collapse of a closed, consistently oriented, edge-manifold mesh (vertices [V,3] fp32, faces [F,3]
     int32; ``marching_tets`` output is one) down to ``target_faces`` faces: rounds of independent collapses
     (``perf_decimate_*``; include/perfb200.h states the rules).  Returns (vertices [V',3], faces [F',3]) with F' = target - 1 or
     target, or more when no collapse is left that keeps the mesh manifold and unfolded.  Faces keep their order and
     orientation, vertices their relative order; repeated runs are byte-identical.  One host read per round.  ``stats``, when a
-    list, receives the number of collapses of every round.  Raises ValueError for a mesh that is not closed and oriented."""
-    if not isinstance(vertices, torch.Tensor) or vertices.dim() != 2 or vertices.shape[1] != 3:
-        raise ValueError(f"decimate: vertices must be [V, 3], got {getattr(vertices, 'shape', type(vertices))}")
-    if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3:
-        raise ValueError(f"decimate: faces must be [F, 3], got {getattr(faces, 'shape', type(faces))}")
+    list, receives the number of collapses of every round.  Raises ValueError for a mesh that is not closed and oriented.
+
+    Topological noise (opt-in, world units): with ``min_component`` the components whose bounding-box diagonal is below it are
+    dropped before the first round and after every cut round; with ``max_cut``, when a round selects no collapse, one cut
+    round cuts the mesh along independent non-face 3-cycles of perimeter <= ``max_cut`` and caps both sides (a handle is
+    removed, or a piece split off), and the collapse rounds go on.  With either set, ``stats`` receives ("collapse" | "cut" |
+    "drop", count) per round: collapses, cuts, components dropped.  Without them the call is exactly the one above."""
+    _check_shapes("decimate", vertices, faces)
     if isinstance(target_faces, bool) or int(target_faces) != target_faces or target_faces < 0:
         raise ValueError(f"decimate: target_faces must be an int >= 0, got {target_faces!r}")
-    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    max_cut, min_component = _check_length("max_cut", max_cut), _check_length("min_component", min_component)
+    vertices, faces = _prepare("decimate", vertices, faces)
+    clean = max_cut is not None or min_component is not None
     V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
-    if V >= 2 ** 31 or 3 * F >= 2 ** 31:
-        raise ValueError(f"decimate: {V} vertices / {F} faces: needs V < 2^31 and 3F < 2^31")
     target = int(target_faces)
     if F == 0:
         return vertices.clone(), faces.clone()
     L = _L()
     with torch.cuda.device(dev):
-        lo, hi = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
-        if lo < 0 or hi >= V:
-            raise ValueError(f"decimate: face indices span [{lo}, {hi}], outside [0, {V})")
-        adj, off = _corner_adjacency(faces, V)
-        flags = torch.zeros(1, dtype=torch.int32, device=dev)
-        _call(L.perf_decimate_check, _p(faces), F, V, _p(adj), _p(off), _p(flags), _stream())
-        bad = int(flags.item())
-        if bad:
-            raise ValueError("decimate: not a closed, consistently oriented, edge-manifold mesh: "
-                             + "; ".join(m for b, m in _DECIMATE_FLAGS.items() if bad & b))
+        adj, off = _check_closed("decimate", faces, V)
         pos, faces = vertices.clone(), faces.clone()
         quad = torch.empty(V, 10, dtype=torch.float64, device=dev)
         _call(L.perf_decimate_quadrics, _p(pos), V, _p(faces), F, _p(adj), _p(off), _p(quad), _stream())
         first = True
+        if min_component is not None:
+            pos, quad, faces, n = _drop_components(pos, quad, faces, min_component)
+            if n:
+                V, F, first = pos.shape[0], faces.shape[0], False
+            if stats is not None:
+                stats.append(("drop", n))
         while F > target:
             if not first:
                 adj, off = _corner_adjacency(faces, V)
@@ -750,7 +868,20 @@ def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, sta
             edges = torch.nonzero(sel).view(-1)                                   # the round's host read
             n = edges.numel()
             if n == 0:
-                break
+                if max_cut is None:
+                    break
+                del key, place, vmin, vmin2, sel
+                pos, quad, faces, n = _cut_round(pos, quad, faces, adj, off, max_cut)
+                if stats is not None:
+                    stats.append(("cut", n))
+                if n == 0:
+                    break
+                if min_component is not None:
+                    pos, quad, faces, d = _drop_components(pos, quad, faces, min_component)
+                    if stats is not None:
+                        stats.append(("drop", d))
+                V, F = pos.shape[0], faces.shape[0]
+                continue
             need = (F - target + 1) // 2
             if n > need:
                 edges = edges[torch.argsort(key[edges])[:need]].contiguous()
@@ -769,7 +900,7 @@ def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, sta
                   _p(pos2), _p(quad2), _p(faces2), _stream(), launches=2)
             pos, quad, faces, V, F = pos2, quad2, faces2, V2, F2
             if stats is not None:
-                stats.append(n)
+                stats.append(("collapse", n) if clean else n)
     return pos, faces
 
 

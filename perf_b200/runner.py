@@ -207,8 +207,10 @@ class CoreRunner:
         and ``mesh_threshold`` (default ``mesh.DEFAULT_THRESHOLD``); with ``mesh_target_faces`` the mesh is decimated to about
         that many faces and written to ``mesh_<res>_f<target>.ply``, so a full mesh is never overwritten.  With
         ``mesh_texture_size`` the colour field is also baked into a texture atlas of that side and the textured mesh written
-        beside the PLY as ``<same stem>.obj`` / ``.mtl`` / ``_albedo.png`` (the PLY is the same either way).  Returns (path,
-        mesh) on rank 0, else (None, None)."""
+        beside the PLY as ``<same stem>.obj`` / ``.mtl`` / ``_albedo.png`` (the PLY is the same either way).  With
+        ``mesh_min_component`` and / or ``mesh_max_cut`` (voxels; ``NeRFScene.extract_mesh``) floaters and short handles are
+        removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  Returns (path, mesh) on rank 0, else
+        (None, None)."""
         from .mesh import write_obj, write_ply
         if not self.is_main:
             return None, None
@@ -217,13 +219,19 @@ class CoreRunner:
         target = self.conf.get("mesh_target_faces", None)
         target = None if target is None else int(target)
         tex = self.conf.get("mesh_texture_size", None)
+        mc, cut = self.conf.get("mesh_min_component", None), self.conf.get("mesh_max_cut", None)
+        clean = {} if mc is None and cut is None else {"min_component": None if mc is None else float(mc),
+                                                       "max_cut": None if cut is None else float(cut)}
         self.set_eval()
         if tex is None:
-            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target)
+            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, **clean)
         else:
-            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, texture_size=int(tex))
+            mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, texture_size=int(tex),
+                                           **clean)
         os.makedirs(pjoin(self.exp_dir, "mesh"), exist_ok=True)
         name = "mesh_{}.ply".format(res) if target is None else "mesh_{}_f{}.ply".format(res, target)
+        if clean:
+            name = name[:-len(".ply")] + "_clean.ply"
         path = pjoin(self.exp_dir, "mesh", name)
         write_ply(path, mesh)
         if tex is not None:
