@@ -398,6 +398,65 @@ int perf_atlas_layout(const float* d_vertices, uint64_t V, const int32_t* d_face
 int perf_atlas_texels(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_face_rec,
                       const int32_t* d_cells, uint64_t C, uint64_t m0, uint64_t n, int32_t* d_face, float* d_point, void* stream);
 
+/* ---- ray casting of a triangle mesh (ops.mesh_bvh / mesh_cast / mesh_shade drive it; csrc/raycast.cu).  d_vertices [V,3] fp32,
+ * d_faces [F,3] int32 (any triangle soup; zero-area faces are never hit).  F < 2^30 and V < 2^31, else PERF_EINVAL.
+ * BVH (Karras 2012 linear BVH, deterministic: two builds of one mesh are byte-identical):
+ *   Codes: per face c = ((p0 + p1) + p2) / 3 in fp32; per axis with ext = hi - lo of the caller's box (the mesh's exact vertex
+ *   min / max), u = fp32(fp32(c - lo) / ext) * 2^21, q = min(2^21 - 1, floor(max(u, 0))), q = 0 when ext = 0; code = the bits
+ *   of qx at 3k, qy at 3k + 1, qz at 3k + 2 (63 bits, int64 >= 0).  The caller sorts (code, face) stably: d_order [F] int32 =
+ *   the face at each leaf position, the sorted codes for the topology.
+ *   Topology: delta(i, j) = clz64(code_i ^ code_j), or 64 + clz32(i ^ j) when the codes are equal, -1 for j outside [0, F);
+ *   internal node i of F - 1 takes Karras's range and split (direction d = sign(delta(i, i+1) - delta(i, i-1)), binary
+ *   searches for the range end and for the split gamma); children gamma and gamma + 1 are leaves when they end the range.
+ *   F = 1: one leaf and no internal node; F = 0: nothing, every ray misses.
+ *   Boxes: exact fp32 min / max, bottom-up, the second thread to reach a node (one atomic counter per node) unites its two
+ *   child boxes, so the result does not depend on arrival order.
+ * Node layout: d_nodes [F - 1, 16] 32-bit words, 64 bytes: words 0-5 the left child's box (lo xyz, hi xyz, fp32), 6-11 the
+ *   right child's, 12 / 13 the left / right child link (c >= 0: internal node c; c < 0: leaf ~c), 14 the parent (-1 at the
+ *   root, node 0), 15 zero.  One 64-byte read decides both children.  d_tris [F, 12] fp32, 48 bytes per leaf in leaf order:
+ *   p0 xyz, the original face id (int32 bits), p1 xyz, 0, p2 xyz, 0 (the face's corners in its own order).
+ *   d_leaf_parent [F] int32 (build only).  Bytes per face: 64 + 48 = 112 for the cast (+ 4 leaf parent, + 8 code and 4 order
+ *   kept by ops.mesh_bvh).
+ * Cast (closest hit): per ray a 16-byte record (t fp32, original face id int32 or -1 on a miss, b1 fp32, b2 fp32); the hit
+ *   point is (1 - b1 - b2) p0 + b1 p1 + b2 p2.  On a miss t = +inf and b1 = b2 = 0.  Only t in [t_min, t_max] counts.  The
+ *   result minimises (t, face id) lexicographically, independently of the traversal order.
+ *   Triangle test: Woop, Benthin & Wald (JCGT 2013), two-sided: kz = the axis of the largest |d| (the first on a tie), kx =
+ *   kz + 1, ky = kx + 1 (mod 3), swapped when d_kz < 0; Sx = d_kx / d_kz, Sy = d_ky / d_kz, Sz = 1 / d_kz; per vertex P = p - o,
+ *   x = P_kx - Sx P_kz, y = P_ky - Sy P_kz; U = cx by - cy bx, V = ax cy - ay cx, W = bx ay - by ax, recomputed in fp64 (then
+ *   rounded to fp32) when any of them is 0; a miss when they have mixed signs or det = (U + V) + W = 0; T = ((U Sz A_kz + V
+ *   Sz B_kz) + W Sz C_kz); t = T / det, b1 = V / det, b2 = W / det.  Each step is one rounded fp32 operation in this order.
+ *   Slab test (conservative; Ize 2013): per axis t0, t1 = (lo - o) / d, (hi - o) / d with the reciprocal 1 / d, widened by
+ *   2^-16 (m / max |d| + |t|), m = the box's largest |lo - o|, |hi - o|; an axis with |d| < 2^-100 is parallel and culls
+ *   only when o lies outside the slab by more than 2^-16 m.  A box is kept when its widened entry is <= the current best t
+ *   (equality kept, for the face-id tie rule).  Traversal: ordered, nearer child first, per-thread stack of 96 entries: the
+ *   common-prefix length delta grows strictly down a Karras tree and is at most 64 + 31.
+ * Shade: from the records, d_rgb [R,3], d_distance [R], d_opacity [R], d_normal [R,3], d_back [R] uint8.  A hit has opacity 1,
+ *   distance t, b0 = (1 - b1) - b2; normal = the blend b0 n0 + b1 n1 + b2 n2 of the vertex normals, normalised (the geometric
+ *   normal (p1 - p0) x (p2 - p0) normalised without d_normals); colour = the blend of the uint8 vertex colours / 255, or with
+ *   d_uv [F,3,2] and d_texture [T,T,3] uint8 (row 0 at v = 1) a bilinear lookup at the blended uv: x = u T - 0.5, y = (1 - v)
+ *   T - 0.5 (texel (x, y) centred at integers), indices clamped to [0, T - 1].  back = d . n_geo > 0.  A miss has opacity 0,
+ *   normal 0, colour 0 and distance 0 before the eval renders' background rule: distance += 5 (1 - opacity), rgb += 0.5 (1 -
+ *   opacity). */
+/* d_codes [F] int64.  h_lo3 / h_hi3: the code box (lo <= hi, finite). */
+int perf_bvh_codes(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const float* h_lo3, const float* h_hi3,
+                   int64_t* d_codes, void* stream);
+/* From the sorted codes: links (words 12-15) of d_nodes [F - 1, 16] and d_leaf_parent [F]. */
+int perf_bvh_topology(const int64_t* d_sorted_codes, uint64_t F, int32_t* d_nodes, int32_t* d_leaf_parent, void* stream);
+/* Boxes (words 0-11) of d_nodes and d_tris [F, 12]; d_counters [F - 1] int32 zeroed by the caller. */
+int perf_bvh_boxes(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_order,
+                   const int32_t* d_leaf_parent, int32_t* d_nodes, float* d_tris, int32_t* d_counters, void* stream);
+/* d_hits [R, 16 bytes] for the rays d_rays_o / d_rays_d [R,3]. */
+int perf_mesh_cast(const int32_t* d_nodes, const float* d_tris, uint64_t F, const float* d_rays_o, const float* d_rays_d, uint64_t R,
+                   float t_min, float t_max, void* d_hits, void* stream);
+/* d_hits [rows, W, 16 bytes] for the rays perf_raygen_pano generates for rows [row0, row0 + rows) of an H x W pano at h_pose;
+ * a warp casts an 8 x 4 pixel patch. */
+int perf_mesh_cast_pano(const int32_t* d_nodes, const float* d_tris, uint64_t F, const float* h_pose, int H, int W, int row0, int rows,
+                        float t_min, float t_max, void* d_hits, void* stream);
+/* d_rays_d [R,3]: the rays' directions (back-face test).  d_colors, d_normals, d_uv / d_texture nullable. */
+int perf_mesh_shade(const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V, const int32_t* d_faces,
+                    uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv, const uint8_t* d_texture, int T,
+                    float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

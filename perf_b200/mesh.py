@@ -249,3 +249,99 @@ def read_obj(path: str) -> dict:
 
 def _np(a) -> np.ndarray:
     return a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
+
+
+_MESH_DTYPES = {"vertices": torch.float32, "faces": torch.int32, "colors": torch.uint8, "normals": torch.float32,
+                "uv": torch.float32, "texture": torch.uint8}
+
+
+def _on_gpu(mesh: dict, device) -> dict:
+    """The mesh arrays render_mesh uses as contiguous CUDA tensors of the kernels' dtypes (numpy arrays of read_ply /
+    read_obj are moved to the GPU)."""
+    out = {}
+    for k, dt in _MESH_DTYPES.items():
+        a = mesh.get(k)
+        if a is None:
+            continue
+        t = a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+        out[k] = t.to(device=device, dtype=dt).contiguous()
+    out["faces"] = out["faces"].reshape(-1, 3)
+    if "uv" in out:
+        out["uv"] = out["uv"].reshape(-1, 3, 2)
+    return out
+
+
+@torch.no_grad()
+def render_mesh(mesh: dict, pose=None, H: Optional[int] = None, W: Optional[int] = None, rays=None, near: float = 0.0,
+                far: float = float("inf"), bvh: Optional[dict] = None, row0: int = 0, rows: Optional[int] = None) -> dict:
+    """Renders a triangle mesh by ray casting on the GPU (``ops.mesh_bvh`` / ``mesh_cast(_pano)`` / ``mesh_shade``): the same
+    outputs as ``NeRFScene.render_pano`` / ``render`` -- {"rgb" [..., 3], "distance" [..., 1], "opacities" [..., 1], "normal"
+    [..., 3]} with the eval renders' background rule -- plus "back" [..., 1] bool, true where the hit face is a back face.
+    ``mesh``: an :func:`extract_mesh` result (with or without texture) or what :func:`read_ply` / :func:`read_obj` return.  Either
+    ``pose`` with ``H``, ``W`` (an equirectangular panorama, rows [row0, row0 + rows)) or ``rays`` ((o, d) or an object with
+    ``.o`` / ``.d``, [..., 3]).  Only hits with t in [near, far] count.  Pass the ``bvh`` of an earlier call (``ops.mesh_bvh``)
+    to render more views of the same mesh without rebuilding it."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    m = _on_gpu(mesh, dev)
+    if bvh is None:
+        bvh = ops.mesh_bvh(m["vertices"], m["faces"])
+    if pose is not None:
+        if H is None or W is None or rays is not None:
+            raise ValueError("render_mesh: a pose needs H and W, and no rays")
+        rows = H - row0 if rows is None else rows
+        hits = ops.mesh_cast_pano(bvh, pose, H, W, row0, rows, near, far, device=dev)
+        _, d = ops.raygen_pano(pose, H, W, row0, rows, device=dev)
+    else:
+        if rays is None:
+            raise ValueError("render_mesh: pass a pose (with H, W) or rays")
+        o, d = (rays.o, rays.d) if hasattr(rays, "o") else rays
+        o, d = o.to(dev, torch.float32).contiguous(), d.to(dev, torch.float32).contiguous()
+        hits = ops.mesh_cast(bvh, o, d, near, far)
+    return ops.mesh_shade(hits, d, m["vertices"], m["faces"], m.get("colors"), m.get("normals"), m.get("uv"), m.get("texture"))
+
+
+def _psnr(a: torch.Tensor, b: torch.Tensor) -> float:
+    mse = float(((a.double() - b.double()) ** 2).mean())
+    return float("inf") if mse == 0 else -10.0 * float(np.log10(mse))
+
+
+@torch.no_grad()
+def compare_to_field(scene, mesh: dict, poses, H: int = 512, W: int = 1024, images: bool = False) -> list:
+    """How well ``mesh`` reproduces the fitted field of ``scene`` (a ``NeRFScene``): per pose, the mesh is rendered with
+    :func:`render_mesh` over the scene's own ray interval (``scene.ray_interval()``) and the field with
+    ``scene.render_pano(..., normals=True)``, both H x W panoramas.  Per pose a dict of
+    ``hit_agreement`` (share of pixels where "mesh hit" equals "field opacity > 0.5"), ``distance_median`` /
+    ``distance_p90`` (|distance difference| where both hit), ``psnr`` (rgb over the whole image, both with the background
+    rule), ``normal_angle_median`` (degrees between the mesh normal and the normalised field normal where both hit) and
+    ``back_face_share`` (share of the mesh hits on back faces: the camera inside the solid, or a wrong orientation).
+    ``images``: also "mesh_rgb", "field_rgb" and "abs_distance" (0 where not both hit) [H, W, C] tensors."""
+    near, far = scene.ray_interval()
+    dev = scene.device
+    m = _on_gpu(mesh, dev)
+    bvh = ops.mesh_bvh(m["vertices"], m["faces"])
+    out = []
+    for pose in poses:
+        pose = torch.as_tensor(pose, dtype=torch.float32)
+        mr = render_mesh(m, pose, H, W, near=near, far=far, bvh=bvh)
+        fr = scene.render_pano(pose, H, W, normals=True)
+        mh = mr["opacities"][..., 0] > 0.5
+        fh = fr["opacities"].reshape(H, W) > 0.5
+        both = mh & fh
+        dd = (mr["distance"][..., 0] - fr["distance"].reshape(H, W)).abs()
+        fn = fr["normal"].reshape(H, W, 3).float()
+        fn_len = fn.norm(dim=-1)
+        ok = both & (fn_len > 0)
+        cos = (mr["normal"] * fn / fn_len.clamp(min=1e-30)[..., None]).sum(-1).clamp(-1.0, 1.0)
+        ang = torch.rad2deg(torch.acos(cos[ok])) if bool(ok.any()) else torch.zeros(0, device=dev)
+        ddb = dd[both]
+        rep = {"hit_agreement": float((mh == fh).float().mean()),
+               "distance_median": float(ddb.median()) if ddb.numel() else float("nan"),
+               "distance_p90": float(torch.quantile(ddb.float()[:1 << 24], 0.9)) if ddb.numel() else float("nan"),
+               "psnr": _psnr(mr["rgb"], fr["rgb"].reshape(H, W, 3)),
+               "normal_angle_median": float(ang.median()) if ang.numel() else float("nan"),
+               "back_face_share": float(mr["back"][..., 0][mh].float().mean()) if bool(mh.any()) else 0.0,
+               "mesh_hits": float(mh.float().mean()), "field_hits": float(fh.float().mean())}
+        if images:
+            rep.update(mesh_rgb=mr["rgb"], field_rgb=fr["rgb"].reshape(H, W, 3), abs_distance=torch.where(both, dd, torch.zeros_like(dd))[..., None])
+        out.append(rep)
+    return out

@@ -1006,6 +1006,112 @@ def atlas_texels(vertices: torch.Tensor, faces: torch.Tensor, atlas: dict, m0: i
     return face, point
 
 
+def mesh_bvh(vertices: torch.Tensor, faces: torch.Tensor) -> dict:
+    """Linear BVH (Karras 2012) of a triangle mesh (vertices [V,3] fp32, faces [F,3] int32) for :func:`mesh_cast`: the code box
+    (the exact vertex min / max), ``perf_bvh_codes``, a stable sort, ``perf_bvh_topology`` and ``perf_bvh_boxes``
+    (include/perfb200.h states the rules and the node layout).  Deterministic: two builds are byte-identical.  Returns an
+    opaque dict of tensors: {"nodes": [F-1,16] int32, "tris": [F,12] fp32, "leaf_parent": [F], "codes": [F] int64 sorted,
+    "order": [F] int32, "F": F}."""
+    _check_shapes("mesh_bvh", vertices, faces)
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
+    if F >= 1 << 30 or V >= 1 << 31:
+        raise ValueError(f"mesh_bvh: {V} vertices / {F} faces: needs V < 2^31 and F < 2^30")
+    L = _L()
+    nodes = torch.zeros(max(F - 1, 0), 16, dtype=torch.int32, device=dev)
+    tris = torch.empty(F, 12, dtype=torch.float32, device=dev)
+    leaf_parent = torch.empty(F, dtype=torch.int32, device=dev)
+    codes = torch.empty(F, dtype=torch.int64, device=dev)
+    order = torch.empty(F, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        if F:
+            lo_i, hi_i = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
+            if lo_i < 0 or hi_i >= V:
+                raise ValueError(f"mesh_bvh: face indices span [{lo_i}, {hi_i}], outside [0, {V})")
+            box = torch.cat([vertices.amin(0), vertices.amax(0)]).tolist()
+            lo, hi = (C.c_float * 3)(*box[:3]), (C.c_float * 3)(*box[3:])
+            _call(L.perf_bvh_codes, _p(vertices), V, _p(faces), F, lo, hi, _p(codes), _stream())
+            codes, perm = torch.sort(codes, stable=True)
+            order = perm.to(torch.int32)
+            _call(L.perf_bvh_topology, _p(codes), F, _p(nodes), _p(leaf_parent), _stream())
+            counters = torch.zeros(max(F - 1, 0), dtype=torch.int32, device=dev)
+            _call(L.perf_bvh_boxes, _p(vertices), V, _p(faces), F, _p(order), _p(leaf_parent), _p(nodes), _p(tris), _p(counters),
+                  _stream())
+    return {"nodes": nodes, "tris": tris, "leaf_parent": leaf_parent, "codes": codes, "order": order, "F": F}
+
+
+def _hits(shape, dev) -> torch.Tensor:
+    return torch.empty(*shape, 4, dtype=torch.int32, device=dev)
+
+
+def mesh_cast(bvh: dict, rays_o: torch.Tensor, rays_d: torch.Tensor, t_min: float = 0.0, t_max: float = math.inf) -> torch.Tensor:
+    """Closest hits of the rays [..., 3] on the mesh of ``bvh`` (:func:`mesh_bvh`): hit records [..., 4] int32 -- column 0 t
+    (fp32 bits), 1 the face id (-1 on a miss), 2 / 3 the barycentrics b1, b2 (fp32 bits); :func:`hit_fields` splits them.
+    Only t in [t_min, t_max] counts; the hit minimises (t, face id) (``perf_mesh_cast``)."""
+    if rays_o.shape != rays_d.shape or rays_o.shape[-1] != 3:
+        raise ValueError(f"mesh_cast: rays must both be [..., 3], got {tuple(rays_o.shape)} and {tuple(rays_d.shape)}")
+    o, d = _chk(rays_o, torch.float32, "rays_o"), _chk(rays_d, torch.float32, "rays_d")
+    hits = _hits(o.shape[:-1], o.device)
+    with torch.cuda.device(o.device):
+        _call(_L().perf_mesh_cast, _p(bvh["nodes"]), _p(bvh["tris"]), bvh["F"], _p(o), _p(d), o.numel() // 3, float(t_min),
+              float(t_max), _p(hits), _stream())
+    return hits
+
+
+def mesh_cast_pano(bvh: dict, pose, H: int, W: int, row0: int = 0, rows: Optional[int] = None, t_min: float = 0.0,
+                   t_max: float = math.inf, device="cuda") -> torch.Tensor:
+    """:func:`mesh_cast` of the rays :func:`raygen_pano` generates for rows [row0, row0 + rows) of an H x W panorama, generated
+    in the kernel and cast in 8 x 4 pixel patches per warp (``perf_mesh_cast_pano``): hit records [rows, W, 4] int32."""
+    rows = H - row0 if rows is None else rows
+    dev = torch.device(device)
+    hits = _hits((rows, W), dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_mesh_cast_pano, _p(bvh["nodes"]), _p(bvh["tris"]), bvh["F"], _pose_array(pose), H, W, row0, rows,
+              float(t_min), float(t_max), _p(hits), _stream())
+    return hits
+
+
+def hit_fields(hits: torch.Tensor):
+    """(t fp32, face int32, b1 fp32, b2 fp32) of hit records [..., 4]."""
+    f = hits.view(torch.float32)
+    return f[..., 0], hits[..., 1], f[..., 2], f[..., 3]
+
+
+def mesh_shade(hits: torch.Tensor, rays_d: torch.Tensor, vertices: torch.Tensor, faces: torch.Tensor, colors=None, normals=None,
+               uv=None, texture=None) -> dict:
+    """The eval renders' outputs from hit records [..., 4] (``perf_mesh_shade``): {"rgb" [..., 3], "distance" [..., 1],
+    "opacities" [..., 1], "normal" [..., 3], "back" [..., 1] bool} with the background rule of the field renders.  Colour:
+    ``colors`` [V,3] uint8 blended, or a bilinear lookup of ``texture`` [T,T,3] uint8 at the blended ``uv`` [F,3,2]; normal:
+    ``normals`` [V,3] blended, else the geometric normal (include/perfb200.h)."""
+    shape = tuple(hits.shape[:-1])
+    hits = _chk(hits, torch.int32, "hits")
+    d = _chk(rays_d, torch.float32, "rays_d")
+    if tuple(d.shape[:-1]) != shape:
+        raise ValueError(f"mesh_shade: rays_d {tuple(d.shape)} does not match hits {tuple(hits.shape)}")
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    colors = None if colors is None else _chk(colors, torch.uint8, "colors")
+    normals = None if normals is None else _chk(normals, torch.float32, "normals")
+    if (uv is None) != (texture is None):
+        raise ValueError("mesh_shade: uv and texture go together")
+    T = 0
+    if texture is not None:
+        uv, texture = _chk(uv, torch.float32, "uv"), _chk(texture, torch.uint8, "texture")
+        if texture.dim() != 3 or texture.shape[0] != texture.shape[1] or texture.shape[2] != 3:
+            raise ValueError(f"mesh_shade: texture must be [T, T, 3], got {tuple(texture.shape)}")
+        T = texture.shape[0]
+    dev = hits.device
+    R = hits.numel() // 4
+    rgb = torch.empty(*shape, 3, dtype=torch.float32, device=dev)
+    dist = torch.empty(*shape, 1, dtype=torch.float32, device=dev)
+    op = torch.empty(*shape, 1, dtype=torch.float32, device=dev)
+    nrm = torch.empty(*shape, 3, dtype=torch.float32, device=dev)
+    back = torch.empty(*shape, 1, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_mesh_shade, _p(hits), _p(d), R, _p(vertices), vertices.shape[0], _p(faces), faces.shape[0], _p(colors),
+              _p(normals), _p(uv), _p(texture), T, _p(rgb), _p(dist), _p(op), _p(nrm), _p(back), _stream())
+    return {"rgb": rgb, "distance": dist, "opacities": op, "normal": nrm, "back": back.bool()}
+
+
 def morton_xy(m: torch.Tensor):
     """(x, y) of Morton indices m (int64): x from the even bits, y from the odd bits."""
     def compact(v):

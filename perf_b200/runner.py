@@ -209,8 +209,9 @@ class CoreRunner:
         ``mesh_texture_size`` the colour field is also baked into a texture atlas of that side and the textured mesh written
         beside the PLY as ``<same stem>.obj`` / ``.mtl`` / ``_albedo.png`` (the PLY is the same either way).  With
         ``mesh_min_component`` and / or ``mesh_max_cut`` (voxels; ``NeRFScene.extract_mesh``) floaters and short handles are
-        removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  Returns (path, mesh) on rank 0, else
-        (None, None)."""
+        removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  With ``mesh_report: true`` the written mesh
+        is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
+        (path, mesh) on rank 0, else (None, None)."""
         from .mesh import write_obj, write_ply
         if not self.is_main:
             return None, None
@@ -236,7 +237,35 @@ class CoreRunner:
         write_ply(path, mesh)
         if tex is not None:
             write_obj(path[:-len(".ply")] + ".obj", mesh)
+        if bool(self.conf.get("mesh_report", False)):
+            self.mesh_report(mesh, path[:-len(".ply")])
         return path, mesh
+
+    @torch.no_grad()
+    def mesh_report(self, mesh, stem, height=512, width=1024):
+        """``mesh.compare_to_field`` of ``mesh`` against the scene at ``height`` x ``width``, from the identity pose (the input
+        panorama) and the pose sampler's anchors with their rotation reset (as ``render_dense`` renders them): writes
+        ``<stem>_report.json`` (per pose the pose and its numbers) and per pose ``<stem>_report_<i>.png``, mesh rgb | field
+        rgb | colourised |distance difference| (where both hit).  Returns the report."""
+        import json
+        from .mesh import compare_to_field
+        poses = [torch.eye(4)]
+        for i in range(self.pose_sampler.n_anchors):
+            pose = self.pose_sampler.sample_pose(i).detach().float().cpu().clone()
+            pose[:3, :3] = torch.eye(3)
+            poses.append(pose)
+        reps = compare_to_field(self.scene, mesh, poses, height, width, images=True)
+        out = []
+        for i, (pose, rep) in enumerate(zip(poses, reps)):
+            dd = rep.pop("abs_distance")[..., 0]
+            heat = torch.from_numpy(np.ascontiguousarray(colorize_single_channel_image(dd)[:, :, ::-1])).to(dd.device).float()
+            row = torch.cat([rep.pop("mesh_rgb").clip(0., 1.) * 255., rep.pop("field_rgb").clip(0., 1.) * 255., heat], 1)
+            write_image("{}_report_{}.png".format(stem, i), row.round().byte())
+            out.append({"pose": pose.tolist(), **rep})
+        report = {"height": height, "width": width, "ray_interval": list(self.scene.ray_interval()), "poses": out}
+        with open(stem + "_report.json", "w") as f:
+            json.dump(report, f, indent=1)
+        return report
 
     @staticmethod
     def _write_video(path, frames, fps=30):

@@ -386,6 +386,7 @@ class NeRFScene:
 
     LOSS_SCALE = 2 ** 7                                               # GradScaler(2**7), never unscaled (nerf.py:139,249-253)
     OCC_STEP = 5e-4                                                   # render_step_size (nerf_renderer.py:151)
+    OCC_NEAR, OCC_FAR = 0.0, 1.5                                      # near_plane / far_plane of the occupancy sampling (nerf_renderer.py:145-151)
 
     def __init__(self, base_exp_dir=".", train_conf=None, estimator_type="fixed", renderer_conf=None,
                  n_samples: int = 128, near: float = 1e-2, far: float = 1.0, device="cuda", writer=None, fused_train: bool = True,
@@ -445,7 +446,7 @@ class NeRFScene:
             # nerf_renderer.py:145-197: occupancy sampling, both fields at every interval (one launch), composite with
             # nerfacc's 1e-4 transmittance cut applied inside (identical to culling first; see csrc/packed.cu)
             est = self.estimator
-            ri, ts, te = ops.occ_sample(est.binaries[0], est._aabb_list(), rays_o.contiguous(), rays_d.contiguous(), 0.0, 1.5,
+            ri, ts, te = ops.occ_sample(est.binaries[0], est._aabb_list(), rays_o.contiguous(), rays_d.contiguous(), self.OCC_NEAR, self.OCC_FAR,
                                         self.OCC_STEP, None)
             out = self.fused.render_occ(rays_o, rays_d, ops.occ_sample.last_offsets, ri, ts, te, early_stop_eps=1e-4, normals=normals)
         else:
@@ -466,6 +467,12 @@ class NeRFScene:
         if normals:
             return self.fused.render_pano(pose, height, width, self.estimator.n_samples, row0=row0, rows=rows, normals=True)
         return self.fused.render_pano(pose, height, width, self.estimator.n_samples, row0=row0, rows=rows)
+
+    def ray_interval(self):
+        """(near, far) of the eval renders' rays: the fixed-S sampler's, or the occupancy sampling's planes."""
+        if self.estimator_type == "occ":
+            return self.OCC_NEAR, self.OCC_FAR
+        return float(self.estimator.near), float(self.estimator.far)
 
     def extract_mesh(self, resolution=512, threshold=None, colors=True, normals=True, target_faces=None, texture_size=None,
                      min_component=None, max_cut=None) -> dict:
@@ -510,7 +517,7 @@ class NeRFScene:
                 # capacity-sized buffers, sample count stays on the device: no host read, graph-capturable (GraphedTrainStep);
                 # a batch without samples is a no-op step here instead of the reference's early return (nerf_renderer.py:156-162)
                 ri, ts, te, offsets, n_dev = ops.occ_sample_static(est.binaries[0], est._aabb_list(), rays_o.float().contiguous(),
-                                                                   rays_d.float().contiguous(), 0.0, 1.5, self.OCC_STEP,
+                                                                   rays_d.float().contiguous(), self.OCC_NEAR, self.OCC_FAR, self.OCC_STEP,
                                                                    jitter if self.nerf.training else None, static)
                 out = ops.fused_packed_train_step(param, rays_o.float(), rays_d.float(), offsets, ri, ts, te, noise, tc, phase, 1e-4, n_dev=n_dev,
                                                   normals=normals)
@@ -519,7 +526,7 @@ class NeRFScene:
                 return {"is_valid": True, "rgb": rgb, "distance": dist, "opacities": op, "dist_loss": _Lazy(lambda: dl.sum() / n_rays),
                         "dist_loss_rays": dl, "dist_loss_inv_n": 1.0 / n_rays, **({"normal": out[4]} if normals else {})}
             ri, ts, te = ops.occ_sample(est.binaries[0], est._aabb_list(), rays_o.float().contiguous(), rays_d.float().contiguous(),
-                                        0.0, 1.5, self.OCC_STEP, jitter if self.nerf.training else None)
+                                        self.OCC_NEAR, self.OCC_FAR, self.OCC_STEP, jitter if self.nerf.training else None)
             if ri.numel() <= 0:                                              # nerf_renderer.py:156-162
                 z = lambda c: torch.zeros(R, c, device=dev)
                 return {"is_valid": False, "rgb": z(3), "distance": z(1), "opacities": z(1), "dist_loss": torch.zeros((), device=dev)}
@@ -780,7 +787,7 @@ class GraphedTrainStep:
             rays, _, _, _ = sup_pool.rand_ray_color_data(R)
             ro, rd = rays.collapse()
             est = scene.estimator
-            probe = ops.occ_sample(est.binaries[0], est._aabb_list(), ro.float().contiguous(), rd.float().contiguous(), 0.0, 1.5,
+            probe = ops.occ_sample(est.binaries[0], est._aabb_list(), ro.float().contiguous(), rd.float().contiguous(), scene.OCC_NEAR, scene.OCC_FAR,
                                    scene.OCC_STEP, torch.rand(R, device=dev))[0].numel()
             cap = occ_capacity or int(max(probe * 1.5, R * 16)) // 128 * 128 + 128
             scene._occ_static = ops.OccStaticBuffers(R, cap, dev)
