@@ -457,6 +457,34 @@ int perf_mesh_shade(const void* d_hits, const float* d_rays_d, uint64_t R, const
                     uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv, const uint8_t* d_texture, int T,
                     float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back, void* stream);
 
+/* ---- texture colour from registered panoramas (ops.texture_views drives it; csrc/texture_views.cu).  One thread per texel
+ * point p of face f = d_face[i] (d_face -1: unused texel); d_face_normal [F,3] the unit geometric normals n (faces point into
+ * free space).  d_views [n_views, H, W] float4 (16-byte aligned): r, g, b in [0, 1] and the distance D, 0 where the view did
+ * not observe the pixel; h_poses [n_views, 16] row-major camera-to-world, rotation R, centre c.  n_views <= 64 (the 12 pose
+ * floats of each view travel in the kernel arguments), else PERF_EINVAL.  Each step below is one rounded fp32 operation in
+ * the order written; dot products are (a0 b0 + a1 b1) + a2 b2.
+ *   Per view v, in registration order: q = p - c, dist2 = q . q; skip v when dist2 = 0; dist = sqrt(dist2).
+ *   Grazing test: cos = -(n . q) / dist (= n . (c - p) / dist); skip v unless cos >= 0.15 (sup_info.py's normal_cos limit).
+ *   Direction: e = (R^T q) / dist per component, e_k = ((R_0k q0 + R_1k q1) + R_2k q2) / dist.  alpha = atan2(e1, e0),
+ *   beta = atan2(e2, sqrt(e0 e0 + e1 e1)); x = (0.5 - alpha * fp32(1 / 2pi)) * W - 0.5, y = (0.5 - beta * fp32(1 / pi)) * H
+ *   - 0.5 (the inverse of common.cuh::pano_dir; pixel centres at integers).
+ *   atan2: t = min(|x|, |y|) / max(|x|, |y|); when t > 0.41421356 (tan pi/8), t = (t - 1) / (t + 1) and pi/4 is added back;
+ *   s = t t, q = ((c9 s + c7) s + c5) s + c3, r = t + (t s) q (c3..c9 in texture_views.cu); r = pi/2 - r when |y| > |x|,
+ *   r = pi - r when x < 0, -r when y < 0; atan2(0, 0) = 0 (fp32 constants).  Max |error| against fp64 arctan2 of the same fp32
+ *   inputs, over 2 M angles at three radii: 2.72e-7 rad (about one ulp of pi), so 1.8e-4 px of x at W = 2048.
+ *   Taps: x0 = floor(x), y0 = floor(y), fx = x - x0, fy = y - y0; columns x0, x0 + 1 wrap modulo W (the seam is continuous on
+ *   the sphere), rows y0, y0 + 1 clamp to [0, H - 1].  Tap weights (1 - fx)(1 - fy), fx (1 - fy), (1 - fx) fy, fx fy in that
+ *   order.  A tap counts when its weight > 0, D > 0 and |dist - D| <= depth_tol (PeRF's visibility test made two-sided: a
+ *   floater in front of an observed wall does not take the wall's colour).  With sw = the sum of the counting weights and
+ *   s = the sum of weight * rgb over them (in tap order), view v counts when sw > 0, its colour rgb_v = s / sw (failed taps
+ *   are dropped, not blended, so silhouettes do not bleed foreground colour onto the background).
+ *   Blend: w_v = cos / dist2; over the views that count, in view order, acc += w_v rgb_v and wsum += w_v.
+ *   Outputs: d_rgb [N,3] = acc / wsum (0 when wsum = 0), d_weight [N] = wsum, d_view [N] int32 = the view with the largest w_v
+ *   (the first on a tie), -1 when no view counts, -2 for an unused texel (rgb and weight 0). */
+int perf_texture_views(const float* d_points, const int32_t* d_face, uint64_t N, const float* d_face_normal, uint64_t F,
+                       const float* d_views, int n_views, int H, int W, const float* h_poses, float depth_tol, float* d_rgb,
+                       float* d_weight, int32_t* d_view, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

@@ -25,7 +25,7 @@ DEFAULT_THRESHOLD = 50.0
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
                  normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None,
-                 min_component: Optional[float] = None, max_cut: Optional[float] = None) -> dict:
+                 min_component: Optional[float] = None, max_cut: Optional[float] = None, texture_views=None) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -34,13 +34,16 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     With ``target_faces`` the mesh is first decimated to about that many faces (``ops.decimate``: quadric-error edge
     collapse, which removes faces where the surface is flat and keeps them where it bends); colours and normals are then the
     fields' at the decimated vertices.  With ``texture_size`` the colour field is then baked into a texture atlas of that side
-    (:func:`bake_texture`): ``"uv"`` [F,3,2] and ``"texture"`` [T,T,3] uint8 join the dict.
+    (:func:`bake_texture`): ``"uv"`` [F,3,2] and ``"texture"`` [T,T,3] uint8 join the dict; with ``texture_views`` (registered
+    panoramas, :func:`bake_texture`'s ``views``) the texels those panoramas see take their colour, and ``"texture_view"`` joins.
     ``min_component`` and ``max_cut`` remove a fit's topological noise, both in voxels of the lattice (the smallest of
     extent / (r - 1) over the axes): components whose bounding-box diagonal is below ``min_component`` are dropped (floaters),
     and with ``target_faces`` the decimation cuts the mesh along non-face 3-cycles of perimeter <= ``max_cut`` where it would
     otherwise stall (short handles through the walls); ``ops.decimate`` states both.  ``max_cut`` needs ``target_faces``."""
     if max_cut is not None and target_faces is None:
         raise ValueError("extract_mesh: max_cut acts on the decimation: it needs target_faces")
+    if texture_views is not None and texture_size is None:
+        raise ValueError("extract_mesh: texture_views colours the texture atlas: it needs texture_size")
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
@@ -66,7 +69,7 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
         if normals:
             out["normals"] = res[2]
     if texture_size is not None:
-        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size))
+        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views))
     return out
 
 
@@ -77,23 +80,40 @@ def _rgb8(rgb16: torch.Tensor) -> torch.Tensor:
 TEXEL_CHUNK = 1 << 24       # texels per perf_atlas_texels / perf_fields_points pass: bounds the working set at 8192^2 and up
 
 
-def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK) -> dict:
+def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK, views=None,
+          depth_tol: float = ops.VIEWS_DEPTH_TOL) -> dict:
     atlas = ops.texture_atlas(verts, faces, size)
     T = atlas["size"]
     image = torch.zeros(T * T, 3, dtype=torch.uint8, device=verts.device)
+    if views is not None:
+        views = _packed_views(views, verts.device)
+        fnormal = ops.face_normals(verts, faces)
+        view_img = torch.full((T * T,), -2, dtype=torch.int32, device=verts.device)
     for m0 in range(0, atlas["used"], chunk):
         n = min(chunk, atlas["used"] - m0)
         face, point = ops.atlas_texels(verts, faces, atlas, m0, n)
         rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
         rgb[face < 0] = 0
         x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=verts.device))
+        if views is not None:
+            vrgb, weight, view = ops.texture_views(point, face, fnormal, views, depth_tol)
+            rgb = torch.where((weight > 0)[:, None], _rgb8(vrgb), rgb)
+            view_img[(T - 1 - y) * T + x] = view
+            del vrgb, weight, view
         image[(T - 1 - y) * T + x] = rgb
         del face, point, rgb, x, y
-    return {"uv": atlas["uv"], "texture": image.view(T, T, 3)}
+    out = {"uv": atlas["uv"], "texture": image.view(T, T, 3)}
+    if views is not None:
+        out["texture_view"] = view_img.view(T, T)
+    return out
+
+
+def _packed_views(views, device) -> dict:
+    return views if isinstance(views, dict) and "data" in views else ops.pack_views(views, device)
 
 
 @torch.no_grad()
-def bake_texture(nerf, mesh: dict, size: int) -> dict:
+def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops.VIEWS_DEPTH_TOL) -> dict:
     """``mesh`` (an :func:`extract_mesh` result) with its colour field baked into a ``size`` x ``size`` texture (a power of two
     in [256, 16384]): adds ``"uv"`` [F,3,2] fp32 (per face corner, v up) and ``"texture"`` [T,T,3] uint8 (row 0 at v = 1).  One
     right-isosceles chart per face, packed in Z-order (``ops.texture_atlas``); each texel holds round(clip(rgb, 0, 1) * 255)
@@ -101,11 +121,17 @@ def bake_texture(nerf, mesh: dict, size: int) -> dict:
     ``perf_fields_points``).  Bilinear lookups at the base level never mix two faces: every texel a lookup inside a chart
     reads belongs to that chart's face.  Mipmaps a viewer builds do mix neighbouring charts at a distance, and texel density
     varies up to about 2x between faces (each chart fills its power-of-two cell).  Raises ValueError when the mesh has more
-    faces than the texture holds (``ops.atlas_face_budget``)."""
+    faces than the texture holds (``ops.atlas_face_budget``).
+    ``views``: registered panoramas (a ``SupInfoPool``, a sequence of (pose, rgb, distance[, mask]) or an ``ops.pack_views``
+    result).  A texel that some panorama sees -- within ``depth_tol`` of its distance map, at a face angle of cos >= 0.15 --
+    then takes the panoramas' colour (``ops.texture_views``: the cos / dist^2 weighted blend of the views that see it) instead
+    of the field's, through the same rounding; the others keep the field's colour.  ``"texture_view"`` [T,T] int32 joins the
+    dict: per texel the view of the largest weight, -1 where the field coloured it, -2 where the texel is unused."""
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
-    return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size))
+    return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size, views=views,
+                              depth_tol=depth_tol))
 
 
 _PLY_PROPS = {"vertices": ("x", "y", "z"), "normals": ("nx", "ny", "nz"), "colors": ("red", "green", "blue")}
@@ -344,4 +370,29 @@ def compare_to_field(scene, mesh: dict, poses, H: int = 512, W: int = 1024, imag
         if images:
             rep.update(mesh_rgb=mr["rgb"], field_rgb=fr["rgb"].reshape(H, W, 3), abs_distance=torch.where(both, dd, torch.zeros_like(dd))[..., None])
         out.append(rep)
+    return out
+
+
+@torch.no_grad()
+def compare_to_views(mesh: dict, views) -> list:
+    """How well ``mesh`` reproduces the registered panoramas ``views`` (a ``SupInfoPool``, a sequence of (pose, rgb,
+    distance[, mask]) or an ``ops.pack_views`` result): each view's pose is rendered with :func:`render_mesh` at the view's own
+    H x W.  Per view a dict of ``hit_share`` (share of the observed pixels -- ``mask_raw``, distance > 0 -- that the mesh
+    hits), ``psnr`` (mesh rgb against the view's colour over the observed pixels the mesh hits) and ``distance_median``
+    (median |mesh distance - view distance| over the same pixels)."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    pv = _packed_views(views, dev)
+    m = _on_gpu(mesh, dev)
+    bvh = ops.mesh_bvh(m["vertices"], m["faces"])
+    Hh, W = pv["data"].shape[1:3]
+    out = []
+    for v in range(pv["data"].shape[0]):
+        mr = render_mesh(m, pv["poses"][v], Hh, W, bvh=bvh)
+        img = pv["data"][v]
+        obs = img[..., 3] > 0
+        sel = obs & (mr["opacities"][..., 0] > 0.5)
+        n_obs, n_sel = int(obs.sum()), int(sel.sum())
+        out.append({"hit_share": n_sel / n_obs if n_obs else float("nan"),
+                    "psnr": _psnr(mr["rgb"][sel], img[..., :3][sel]) if n_sel else float("nan"),
+                    "distance_median": float((mr["distance"][..., 0][sel] - img[..., 3][sel]).abs().median()) if n_sel else float("nan")})
     return out

@@ -1112,6 +1112,84 @@ def mesh_shade(hits: torch.Tensor, rays_d: torch.Tensor, vertices: torch.Tensor,
     return {"rgb": rgb, "distance": dist, "opacities": op, "normal": nrm, "back": back.bool()}
 
 
+VIEWS_MAX = 64              # perf_texture_views carries the poses in its kernel arguments
+# |dist - D| a panorama pixel may differ from the texel point's distance and still colour it (DESIGN.md section 6: the sweep
+# over {0.005, 0.01, 0.02, 0.04} on the fitted box room)
+VIEWS_DEPTH_TOL = 0.02
+
+
+def pack_views(source, device=None) -> dict:
+    """The registered panoramas as :func:`texture_views` reads them: ``{"data": [n,H,W,4] fp32 (r, g, b, distance; the
+    distance 0 where the pixel is not observed), "poses": [n,4,4] fp32 camera-to-world (host)}``.  ``source`` is a
+    ``SupInfoPool`` (each panorama's ``pose``, ``color_map``, ``distance_map`` and ``mask_raw``) or a sequence of
+    ``(pose, rgb [H,W,3], distance [H,W(,1)][, mask [H,W(,1)]])`` (without a mask, observed = distance > 0).  Raises ValueError
+    on panoramas of different sizes, none, or more than 64."""
+    if hasattr(source, "sup_infos"):
+        items = [(i.pose, i.color_map, i.distance_map, i.mask_raw) for i in source.sup_infos]
+    else:
+        items = [tuple(s) for s in source]
+    if not items or len(items) > VIEWS_MAX:
+        raise ValueError(f"pack_views: {len(items)} panoramas: needs 1 to {VIEWS_MAX}")
+    rgb0 = items[0][1]
+    Hh, W = int(rgb0.shape[0]), int(rgb0.shape[1])
+    dev = torch.device(device) if device is not None else (rgb0.device if torch.is_tensor(rgb0) and rgb0.is_cuda
+                                                           else torch.device("cuda", torch.cuda.current_device()))
+    data = torch.empty(len(items), Hh, W, 4, dtype=torch.float32, device=dev)
+    poses = torch.empty(len(items), 4, 4, dtype=torch.float32)
+    for v, it in enumerate(items):
+        if len(it) not in (3, 4):
+            raise ValueError("pack_views: each view is (pose, rgb, distance[, mask])")
+        pose, rgb, dist = it[:3]
+        rgb, dist = torch.as_tensor(rgb).to(dev, torch.float32), torch.as_tensor(dist).to(dev, torch.float32)
+        if tuple(rgb.shape) != (Hh, W, 3) or dist.numel() != Hh * W:
+            raise ValueError(f"pack_views: view {v} is {tuple(rgb.shape)} / {tuple(dist.shape)}, view 0 is ({Hh}, {W}, 3): all views "
+                             "must share one size")
+        dist = dist.reshape(Hh, W)
+        mask = dist > 0 if len(it) == 3 else torch.as_tensor(it[3]).to(dev).reshape(Hh, W).bool() & (dist > 0)
+        data[v, :, :, :3] = rgb
+        data[v, :, :, 3] = torch.where(mask, dist, torch.zeros_like(dist))
+        poses[v] = torch.as_tensor(pose, dtype=torch.float32).detach().cpu().reshape(4, 4)
+    return {"data": data, "poses": poses}
+
+
+def face_normals(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:
+    """Unit geometric normals [F,3] fp32, (p1 - p0) x (p2 - p0) normalised (0 for a zero-area face): the normal
+    ``perf_mesh_shade`` shades with when the mesh has no vertex normals."""
+    p = vertices[faces.long()]
+    n = torch.linalg.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0])
+    nn = n.norm(dim=-1, keepdim=True)
+    return torch.where(nn > 0, n / nn.clamp(min=1e-30), torch.zeros_like(n)).contiguous()
+
+
+def texture_views(points: torch.Tensor, face: torch.Tensor, face_normals: torch.Tensor, views: dict,
+                  depth_tol: float = VIEWS_DEPTH_TOL):
+    """Colour of texel points [N,3] (faces ``face`` [N] int32, -1 unused; unit ``face_normals`` [F,3]) projected into the
+    panoramas of ``views`` (:func:`pack_views`) with a two-sided depth test of ``depth_tol`` world units:
+    ``perf_texture_views`` (include/perfb200.h states the rule).  Returns (rgb [N,3] fp32, the cos / dist^2 weighted blend of
+    the views that see the point; weight [N] fp32, the sum of those weights, 0 where no view sees it; view [N] int32, the
+    view of the largest weight, -1 where none, -2 for an unused texel)."""
+    points, face = _chk(points, torch.float32, "points"), _chk(face, torch.int32, "face")
+    face_normals = _chk(face_normals, torch.float32, "face_normals")
+    data = _chk(views["data"], torch.float32, "views")
+    if data.dim() != 4 or data.shape[-1] != 4 or not 1 <= data.shape[0] <= VIEWS_MAX:
+        raise ValueError(f"texture_views: views must be [n <= {VIEWS_MAX}, H, W, 4], got {tuple(data.shape)}")
+    poses = torch.as_tensor(views["poses"], dtype=torch.float32).detach().cpu().reshape(-1, 16)
+    if poses.shape[0] != data.shape[0]:
+        raise ValueError(f"texture_views: {poses.shape[0]} poses for {data.shape[0]} views")
+    N, dev = face.shape[0], points.device
+    if tuple(points.shape) != (N, 3) or face_normals.dim() != 2 or face_normals.shape[1] != 3:
+        raise ValueError(f"texture_views: points {tuple(points.shape)}, face {tuple(face.shape)}, face_normals "
+                         f"{tuple(face_normals.shape)}: needs [N,3], [N], [F,3]")
+    rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+    weight = torch.empty(N, dtype=torch.float32, device=dev)
+    view = torch.empty(N, dtype=torch.int32, device=dev)
+    h = (C.c_float * poses.numel())(*poses.reshape(-1).tolist())
+    with torch.cuda.device(dev):
+        _call(_L().perf_texture_views, _p(points), _p(face), N, _p(face_normals), face_normals.shape[0], _p(data), data.shape[0],
+              data.shape[1], data.shape[2], h, float(depth_tol), _p(rgb), _p(weight), _p(view), _stream())
+    return rgb, weight, view
+
+
 def morton_xy(m: torch.Tensor):
     """(x, y) of Morton indices m (int64): x from the even bits, y from the odd bits."""
     def compact(v):

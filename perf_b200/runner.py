@@ -208,6 +208,9 @@ class CoreRunner:
         that many faces and written to ``mesh_<res>_f<target>.ply``, so a full mesh is never overwritten.  With
         ``mesh_texture_size`` the colour field is also baked into a texture atlas of that side and the textured mesh written
         beside the PLY as ``<same stem>.obj`` / ``.mtl`` / ``_albedo.png`` (the PLY is the same either way).  With
+        ``mesh_texture_views: true`` (needs ``mesh_texture_size``) the texels that a registered panorama of ``self.sup_pool``
+        sees take the panoramas' colour instead of the field's (``mesh.bake_texture``'s ``views``), and the OBJ set is written
+        as ``<stem>_views.obj`` / ``.mtl`` / ``_views_albedo.png``; the PLY and its vertex colours stay the field's.  With
         ``mesh_min_component`` and / or ``mesh_max_cut`` (voxels; ``NeRFScene.extract_mesh``) floaters and short handles are
         removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  With ``mesh_report: true`` the written mesh
         is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
@@ -220,9 +223,14 @@ class CoreRunner:
         target = self.conf.get("mesh_target_faces", None)
         target = None if target is None else int(target)
         tex = self.conf.get("mesh_texture_size", None)
+        views = bool(self.conf.get("mesh_texture_views", False))
+        if views and tex is None:
+            raise ValueError("mesh_texture_views colours the texture atlas: it needs mesh_texture_size")
         mc, cut = self.conf.get("mesh_min_component", None), self.conf.get("mesh_max_cut", None)
         clean = {} if mc is None and cut is None else {"min_component": None if mc is None else float(mc),
                                                        "max_cut": None if cut is None else float(cut)}
+        if views:
+            clean["texture_views"] = self.sup_pool
         self.set_eval()
         if tex is None:
             mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, **clean)
@@ -231,24 +239,26 @@ class CoreRunner:
                                            **clean)
         os.makedirs(pjoin(self.exp_dir, "mesh"), exist_ok=True)
         name = "mesh_{}.ply".format(res) if target is None else "mesh_{}_f{}.ply".format(res, target)
-        if clean:
+        if mc is not None or cut is not None:
             name = name[:-len(".ply")] + "_clean.ply"
         path = pjoin(self.exp_dir, "mesh", name)
         write_ply(path, mesh)
         if tex is not None:
-            write_obj(path[:-len(".ply")] + ".obj", mesh)
+            write_obj(path[:-len(".ply")] + ("_views.obj" if views else ".obj"), mesh)
         if bool(self.conf.get("mesh_report", False)):
-            self.mesh_report(mesh, path[:-len(".ply")])
+            self.mesh_report(mesh, path[:-len(".ply")], views=self.sup_pool if views else None)
         return path, mesh
 
     @torch.no_grad()
-    def mesh_report(self, mesh, stem, height=512, width=1024):
+    def mesh_report(self, mesh, stem, height=512, width=1024, views=None):
         """``mesh.compare_to_field`` of ``mesh`` against the scene at ``height`` x ``width``, from the identity pose (the input
         panorama) and the pose sampler's anchors with their rotation reset (as ``render_dense`` renders them): writes
         ``<stem>_report.json`` (per pose the pose and its numbers) and per pose ``<stem>_report_<i>.png``, mesh rgb | field
-        rgb | colourised |distance difference| (where both hit).  Returns the report."""
+        rgb | colourised |distance difference| (where both hit).  With ``views`` (registered panoramas, the ones the texture
+        was coloured from) the JSON also gets ``"views"``, ``mesh.compare_to_views`` per panorama, and
+        ``"views_texel_share"``, the share of the used texels that the panoramas coloured.  Returns the report."""
         import json
-        from .mesh import compare_to_field
+        from .mesh import compare_to_field, compare_to_views
         poses = [torch.eye(4)]
         for i in range(self.pose_sampler.n_anchors):
             pose = self.pose_sampler.sample_pose(i).detach().float().cpu().clone()
@@ -263,6 +273,11 @@ class CoreRunner:
             write_image("{}_report_{}.png".format(stem, i), row.round().byte())
             out.append({"pose": pose.tolist(), **rep})
         report = {"height": height, "width": width, "ray_interval": list(self.scene.ray_interval()), "poses": out}
+        if views is not None:
+            report["views"] = compare_to_views(mesh, views)
+            tv = mesh["texture_view"]
+            used = int((tv != -2).sum())
+            report["views_texel_share"] = int((tv >= 0).sum()) / used if used else 0.0
         with open(stem + "_report.json", "w") as f:
             json.dump(report, f, indent=1)
         return report
