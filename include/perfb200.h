@@ -457,6 +457,40 @@ int perf_mesh_shade(const void* d_hits, const float* d_rays_d, uint64_t R, const
                     uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv, const uint8_t* d_texture, int T,
                     float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back, void* stream);
 
+/* ---- normal texture of a decimated mesh (ops.bake_normal_texture / mesh_shade drive it; csrc/raycast.cu).  The low mesh
+ * (d_vertices, d_faces, d_normals nullable, d_uv [F,3,2] its atlas, perf_atlas_layout) gets a tangent-space normal texture of
+ * the high mesh (the full-resolution surface, d_hi_*, with its BVH from perf_bvh_*).  Each step is one rounded fp32 operation
+ * in the order written; dot products are (a0 b0 + a1 b1) + a2 b2, cross products a x b = (a1 b2 - a2 b1, a2 b0 - a0 b2,
+ * a0 b1 - a1 b0).
+ *   Barycentrics of texel point p on its low face f: e1 = p1 - p0, e2 = p2 - p0, q = p - p0, g = e1 x e2, G = g . g;
+ *   b1 = ((q x e2) . g) / G, b2 = ((e1 x q) . g) / G, b0 = (1 - b1) - b2.  G = 0: the flat texel, offset +inf.
+ *   Casts: from p along +g^ and -g^ (g^ = g / sqrt(G)), t in [0, distance], the cast of perf_mesh_cast; the hit is the one of
+ *   smaller t, +g^ on a tie; offset = +t or -t, +inf when neither ray hits (then the flat texel).
+ *   High normal N at the hit: perf_mesh_shade's normal rule on the high mesh (blend of d_hi_normals normalised, else the
+ *   geometric normal normalised).
+ *   Frame (MikkTSpace for per-face charts: no corner is welded across faces): du_k = u_k - u0, dv_k = v_k - v0 (k = 1, 2),
+ *   T_f = (dv2 e1 - dv1 e2) / (du1 dv2 - du2 dv1) per component; per corner n_k = the vertex normal (the unit geometric normal
+ *   g^ without d_normals), t_k = T_f - n_k (n_k . T_f) normalised (0 when it is 0); n = (b0 n0 + b1 n1) + b2 n2 and t likewise,
+ *   unnormalised; b = n x t (sign +1: every chart has positive signed area in uv).
+ *   Encode: det = t . (b x n); flat when !(|det| > ((1e-12 |t|) |b|) |n|); c = (N . (b x n), t . (N x n), t . (b x N)) / det,
+ *   normalised (flat when |c| = 0); texel = clamp(floor((c + 1) 127.5 + 0.5), 0, 255) per channel, RGB8 (+G = +v, OpenGL /
+ *   glTF).  Flat texel: (128, 128, 255), also for an unused texel (d_face -1, offset +inf).
+ *   Shade (perf_mesh_shade_normal_texture): perf_mesh_shade with, after the normal, a bilinear lookup of d_normal_texture
+ *   [T,T,3] at the blended uv with the albedo's addressing, per channel on the bytes: top = (1 - fx) s00 + fx s10, bottom
+ *   likewise, s = (1 - fy) top + fy bottom; c = s / 127.5 - 1; normal = ((c0 t + c1 b) + c2 n) normalised with the frame at the
+ *   hit's barycentrics, or the normal without the texture when that vector is 0. */
+/* d_texel [N,3] uint8 and d_offset [N] fp32 for the texels d_face [N] / d_point [N,3] of perf_atlas_texels; distance finite
+ * and >= 0. */
+int perf_normal_texture_bake(const int32_t* d_nodes, const float* d_tris, const float* d_hi_vertices, uint64_t hi_V,
+                             const int32_t* d_hi_faces, uint64_t hi_F, const float* d_hi_normals, const float* d_vertices, uint64_t V,
+                             const int32_t* d_faces, uint64_t F, const float* d_normals, const float* d_uv, const int32_t* d_face,
+                             const float* d_point, uint64_t N, float distance, uint8_t* d_texel, float* d_offset, void* stream);
+/* perf_mesh_shade's arguments plus d_normal_texture [T,T,3] uint8 (needs d_uv; d_texture nullable, of the same side T). */
+int perf_mesh_shade_normal_texture(const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V,
+                                   const int32_t* d_faces, uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv,
+                                   const uint8_t* d_texture, const uint8_t* d_normal_texture, int T, float* d_rgb, float* d_distance,
+                                   float* d_opacity, float* d_normal, uint8_t* d_back, void* stream);
+
 /* ---- texture colour from registered panoramas (ops.texture_views drives it; csrc/texture_views.cu).  One thread per texel
  * point p of face f = d_face[i] (d_face -1: unused texel); d_face_normal [F,3] the unit geometric normals n (faces point into
  * free space).  d_views [n_views, H, W] float4 (16-byte aligned): r, g, b in [0, 1] and the distance D, 0 where the view did

@@ -363,6 +363,7 @@ struct ShadeArgs {
     const float* uv;                                // [F,3,2] nullable (with texture)
     const uint8_t* texture; int T;                  // [T,T,3]
     float* rgb; float* dist; float* op; float* nrm; uint8_t* back;
+    const uint8_t* ntex;                            // [T,T,3] normal texture (shade_ray<true> only)
 };
 
 __host__ __device__ __forceinline__ float shade_texel(const ShadeArgs& a, int x, int y, int c)
@@ -371,7 +372,129 @@ __host__ __device__ __forceinline__ float shade_texel(const ShadeArgs& a, int x,
     y = y < 0 ? 0 : (y >= a.T ? a.T - 1 : y);
     return (float)a.texture[3 * ((int64_t)y * a.T + x) + c];
 }
+// The same addressing in the normal texture.
+__host__ __device__ __forceinline__ float shade_ntexel(const ShadeArgs& a, int x, int y, int c)
+{
+    x = x < 0 ? 0 : (x >= a.T ? a.T - 1 : x);
+    y = y < 0 ? 0 : (y >= a.T ? a.T - 1 : y);
+    return (float)a.ntex[3 * ((int64_t)y * a.T + x) + c];
+}
 
+// The shading normal of a hit at barycentrics w on the face of vertices v and geometric normal g = (p1 - p0) x (p2 - p0):
+// the blend of the vertex normals, or g without them, normalised (0 when the blend is 0).  The mesh shade and the normal
+// texture bake (the normal of the full-resolution surface it encodes) share it.
+__host__ __device__ __forceinline__ void shade_normal(const float* normals, const int32_t (&v)[3], const float (&g)[3],
+                                                      const float (&w)[3], float (&n)[3])
+{
+    for (int d = 0; d < 3; ++d) {
+        n[d] = g[d];
+        if (normals)
+            n[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], normals[3 * (int64_t)v[0] + d]),
+                                             PERF_FMUL_RN(w[1], normals[3 * (int64_t)v[1] + d])),
+                                PERF_FMUL_RN(w[2], normals[3 * (int64_t)v[2] + d]));
+    }
+    const float nn = PERF_FSQRT_RN(PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(n[0], n[0]), PERF_FMUL_RN(n[1], n[1])), PERF_FMUL_RN(n[2], n[2])));
+    for (int d = 0; d < 3; ++d) n[d] = nn > 0.0f ? PERF_FDIV_RN(n[d], nn) : 0.0f;
+}
+
+// ---------------------------------------------------------------- normal texture (perfb200.h, perf_normal_texture_bake)
+__host__ __device__ __forceinline__ float nt_dot(const float (&a)[3], const float (&b)[3])
+{
+    return PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(a[0], b[0]), PERF_FMUL_RN(a[1], b[1])), PERF_FMUL_RN(a[2], b[2]));
+}
+__host__ __device__ __forceinline__ void nt_cross(const float (&a)[3], const float (&b)[3], float (&c)[3])
+{
+    c[0] = PERF_FSUB_RN(PERF_FMUL_RN(a[1], b[2]), PERF_FMUL_RN(a[2], b[1]));
+    c[1] = PERF_FSUB_RN(PERF_FMUL_RN(a[2], b[0]), PERF_FMUL_RN(a[0], b[2]));
+    c[2] = PERF_FSUB_RN(PERF_FMUL_RN(a[0], b[1]), PERF_FMUL_RN(a[1], b[0]));
+}
+
+// MikkTSpace's frame for per-face charts (no corner is welded across faces) at barycentrics w of a face with edges e1, e2,
+// geometric normal g = e1 x e2 and corner uv[6]: the face tangent T_f from the uv differences, per corner t_k = T_f made
+// orthogonal to n_k (the vertex normal, or the unit geometric normal without vertex normals) and normalised, then the
+// unnormalised blends n = sum w_k n_k, t = sum w_k t_k and the bitangent b = n x t (sign +1: every chart has positive area).
+__host__ __device__ __forceinline__ void nt_frame(const float (&e1)[3], const float (&e2)[3], const float (&g)[3], const float* normals,
+                                                  const int32_t (&v)[3], const float* uv, const float (&w)[3], float (&t)[3],
+                                                  float (&b)[3], float (&n)[3])
+{
+    const float du1 = PERF_FSUB_RN(uv[2], uv[0]), dv1 = PERF_FSUB_RN(uv[3], uv[1]);
+    const float du2 = PERF_FSUB_RN(uv[4], uv[0]), dv2 = PERF_FSUB_RN(uv[5], uv[1]);
+    const float den = PERF_FSUB_RN(PERF_FMUL_RN(du1, dv2), PERF_FMUL_RN(du2, dv1));
+    float tf[3], gh[3];
+    for (int d = 0; d < 3; ++d) tf[d] = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FMUL_RN(dv2, e1[d]), PERF_FMUL_RN(dv1, e2[d])), den);
+    const float gl = PERF_FSQRT_RN(nt_dot(g, g));
+    for (int d = 0; d < 3; ++d) gh[d] = gl > 0.0f ? PERF_FDIV_RN(g[d], gl) : 0.0f;
+    float nk[3][3], tk[3][3];
+    for (int k = 0; k < 3; ++k) {
+        float u[3];
+        for (int d = 0; d < 3; ++d) nk[k][d] = normals ? normals[3 * (int64_t)v[k] + d] : gh[d];
+        const float s = nt_dot(nk[k], tf);
+        for (int d = 0; d < 3; ++d) u[d] = PERF_FSUB_RN(tf[d], PERF_FMUL_RN(nk[k][d], s));
+        const float ul = PERF_FSQRT_RN(nt_dot(u, u));
+        for (int d = 0; d < 3; ++d) tk[k][d] = ul > 0.0f ? PERF_FDIV_RN(u[d], ul) : 0.0f;
+    }
+    for (int d = 0; d < 3; ++d) {
+        n[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], nk[0][d]), PERF_FMUL_RN(w[1], nk[1][d])), PERF_FMUL_RN(w[2], nk[2][d]));
+        t[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], tk[0][d]), PERF_FMUL_RN(w[1], tk[1][d])), PERF_FMUL_RN(w[2], tk[2][d]));
+    }
+    nt_cross(n, t, b);
+}
+
+// Encodes the unit normal N in the frame (t, b, n): c = [t b n]^-1 N by Cramer's rule, normalised, stored as
+// floor((c + 1) 127.5 + 0.5) clamped to [0, 255].  False (the caller keeps the flat texel) for a degenerate frame,
+// |det| <= 1e-12 |t| |b| |n|, or c = 0.
+__host__ __device__ __forceinline__ bool nt_encode(const float (&t)[3], const float (&b)[3], const float (&n)[3], const float (&N)[3],
+                                                   uint8_t* out)
+{
+    float bn[3], Nn[3], bN[3];
+    nt_cross(b, n, bn);
+    const float det = nt_dot(t, bn);
+    const float lim = PERF_FMUL_RN(PERF_FMUL_RN(PERF_FMUL_RN(1e-12f, PERF_FSQRT_RN(nt_dot(t, t))), PERF_FSQRT_RN(nt_dot(b, b))),
+                                   PERF_FSQRT_RN(nt_dot(n, n)));
+    if (!(fabsf(det) > lim)) return false;
+    nt_cross(N, n, Nn);
+    nt_cross(b, N, bN);
+    const float c[3] = {PERF_FDIV_RN(nt_dot(N, bn), det), PERF_FDIV_RN(nt_dot(t, Nn), det), PERF_FDIV_RN(nt_dot(t, bN), det)};
+    const float cl = PERF_FSQRT_RN(nt_dot(c, c));
+    if (!(cl > 0.0f)) return false;
+    for (int k = 0; k < 3; ++k) {
+        const float q = floorf(PERF_FADD_RN(PERF_FMUL_RN(PERF_FADD_RN(PERF_FDIV_RN(c[k], cl), 1.0f), 127.5f), 0.5f));
+        out[k] = (uint8_t)(q < 0.0f ? 0.0f : (q > 255.0f ? 255.0f : q));
+    }
+    return true;
+}
+
+// The normal texture applied to a hit (the shading normal n of shade_normal on input): a bilinear lookup of the bytes at
+// the blended uv with the albedo's addressing, c = texel / 127.5 - 1, n = normalise((c.x t + c.y b) + c.z n_frame); n is
+// left as it is when that vector is 0 (a degenerate frame).
+__host__ __device__ __forceinline__ void shade_normal_texture(const ShadeArgs& a, int32_t f, const float (&e1)[3], const float (&e2)[3],
+                                                              const float (&g)[3], const int32_t (&v)[3], const float (&w)[3],
+                                                              float (&n)[3])
+{
+    const float* uv = a.uv + 6 * (int64_t)f;
+    const float u = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], uv[0]), PERF_FMUL_RN(w[1], uv[2])), PERF_FMUL_RN(w[2], uv[4]));
+    const float vv = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], uv[1]), PERF_FMUL_RN(w[1], uv[3])), PERF_FMUL_RN(w[2], uv[5]));
+    const float T = (float)a.T;
+    const float x = PERF_FSUB_RN(PERF_FMUL_RN(u, T), 0.5f), y = PERF_FSUB_RN(PERF_FMUL_RN(PERF_FSUB_RN(1.0f, vv), T), 0.5f);
+    const float x0 = floorf(x), y0 = floorf(y), fx = PERF_FSUB_RN(x, x0), fy = PERF_FSUB_RN(y, y0);
+    const int ix = (int)x0, iy = (int)y0;
+    float c[3], t[3], b[3], m[3], N[3];
+    for (int k = 0; k < 3; ++k) {
+        const float top = PERF_FADD_RN(PERF_FMUL_RN(PERF_FSUB_RN(1.0f, fx), shade_ntexel(a, ix, iy, k)),
+                                       PERF_FMUL_RN(fx, shade_ntexel(a, ix + 1, iy, k)));
+        const float bot = PERF_FADD_RN(PERF_FMUL_RN(PERF_FSUB_RN(1.0f, fx), shade_ntexel(a, ix, iy + 1, k)),
+                                       PERF_FMUL_RN(fx, shade_ntexel(a, ix + 1, iy + 1, k)));
+        c[k] = PERF_FSUB_RN(PERF_FDIV_RN(PERF_FADD_RN(PERF_FMUL_RN(PERF_FSUB_RN(1.0f, fy), top), PERF_FMUL_RN(fy, bot)), 127.5f), 1.0f);
+    }
+    nt_frame(e1, e2, g, a.normals, v, uv, w, t, b, m);
+    for (int d = 0; d < 3; ++d)
+        N[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(c[0], t[d]), PERF_FMUL_RN(c[1], b[d])), PERF_FMUL_RN(c[2], m[d]));
+    const float nl = PERF_FSQRT_RN(nt_dot(N, N));
+    if (nl > 0.0f)
+        for (int d = 0; d < 3; ++d) n[d] = PERF_FDIV_RN(N[d], nl);
+}
+
+template <bool NT>
 __host__ __device__ __forceinline__ void shade_ray(const ShadeArgs& a, int64_t i)
 {
     const float4 h = a.hits[i];
@@ -397,15 +520,8 @@ __host__ __device__ __forceinline__ void shade_ray(const ShadeArgs& a, int64_t i
         const float* dir = a.d + 3 * i;
         const float dg = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(dir[0], g[0]), PERF_FMUL_RN(dir[1], g[1])), PERF_FMUL_RN(dir[2], g[2]));
         back = dg > 0.0f;
-        for (int d = 0; d < 3; ++d) {
-            n[d] = g[d];
-            if (a.normals)
-                n[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], a.normals[3 * (int64_t)v[0] + d]),
-                                                 PERF_FMUL_RN(w[1], a.normals[3 * (int64_t)v[1] + d])),
-                                    PERF_FMUL_RN(w[2], a.normals[3 * (int64_t)v[2] + d]));
-        }
-        const float nn = PERF_FSQRT_RN(PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(n[0], n[0]), PERF_FMUL_RN(n[1], n[1])), PERF_FMUL_RN(n[2], n[2])));
-        for (int d = 0; d < 3; ++d) n[d] = nn > 0.0f ? PERF_FDIV_RN(n[d], nn) : 0.0f;
+        shade_normal(a.normals, v, g, w, n);
+        if (NT) shade_normal_texture(a, f, e1, e2, g, v, w, n);
         if (a.texture) {
             // texel (x, y) of row y (row 0 at v = 1) has its centre at u = (x + 0.5) / T, v = 1 - (y + 0.5) / T
             const float* uv = a.uv + 6 * (int64_t)f;
@@ -436,6 +552,78 @@ __host__ __device__ __forceinline__ void shade_ray(const ShadeArgs& a, int64_t i
     a.dist[i] = PERF_FADD_RN(dist, PERF_FMUL_RN(5.0f, miss));
     a.op[i] = op;
     a.back[i] = back;
+}
+
+// ---------------------------------------------------------------- normal texture bake
+struct BakeArgs {
+    const int32_t* nodes; const float* tris; int64_t hF;  // the high mesh's BVH
+    const float* hpos; const int32_t* hfaces; const float* hnormals;  // the high mesh ([V,3] normals nullable)
+    const float* pos; const int32_t* faces; const float* normals; const float* uv;  // the low mesh (normals nullable)
+    const int32_t* face; const float* point; int64_t N;  // the texels (perf_atlas_texels)
+    float dist;
+    uint8_t* texel; float* offset;
+};
+
+__host__ __device__ __forceinline__ void load_face(const float* pos, const int32_t* faces, int32_t f, int32_t (&v)[3], float (&p)[3][3],
+                                                   float (&e1)[3], float (&e2)[3], float (&g)[3])
+{
+    for (int k = 0; k < 3; ++k) {
+        v[k] = faces[3 * (int64_t)f + k];
+        for (int d = 0; d < 3; ++d) p[k][d] = pos[3 * (int64_t)v[k] + d];
+    }
+    for (int d = 0; d < 3; ++d) { e1[d] = PERF_FSUB_RN(p[1][d], p[0][d]); e2[d] = PERF_FSUB_RN(p[2][d], p[0][d]); }
+    nt_cross(e1, e2, g);
+}
+
+// Texel i: barycentrics of its point on its low face, casts along +g and -g (unit geometric normal) over [0, dist] into the
+// high mesh, the high mesh's shading normal at the nearer hit (+g on a tie), encoded in the low face's frame.
+__host__ __device__ __forceinline__ void bake_texel(const BakeArgs& a, int64_t i)
+{
+    uint8_t out[3] = {128, 128, 255};
+    float off = INFINITY;
+    const int32_t f = a.face[i];
+    int32_t v[3];
+    float p[3][3], e1[3], e2[3], g[3];
+    if (f >= 0) load_face(a.pos, a.faces, f, v, p, e1, e2, g);
+    const float G = f >= 0 ? nt_dot(g, g) : 0.0f;
+    if (G > 0.0f) {
+        float q[3], qe2[3], e1q[3];
+        for (int d = 0; d < 3; ++d) q[d] = PERF_FSUB_RN(a.point[3 * i + d], p[0][d]);
+        nt_cross(q, e2, qe2);
+        nt_cross(e1, q, e1q);
+        const float b1 = PERF_FDIV_RN(nt_dot(qe2, g), G), b2 = PERF_FDIV_RN(nt_dot(e1q, g), G);
+        const float w[3] = {PERF_FSUB_RN(PERF_FSUB_RN(1.0f, b1), b2), b1, b2};
+        const float gl = PERF_FSQRT_RN(G);
+        float gh[3];
+        for (int d = 0; d < 3; ++d) gh[d] = PERF_FDIV_RN(g[d], gl);
+        // one cast at a time: a single call site keeps one traversal stack in the frame
+        float4 best = make_float4(INFINITY, bvh_f(-1), 0.0f, 0.0f);
+        int side = 0;
+#pragma unroll 1
+        for (int s = 0; s < 2; ++s) {
+            Ray r;
+            for (int d = 0; d < 3; ++d) { r.o[d] = a.point[3 * i + d]; r.d[d] = s ? -gh[d] : gh[d]; }
+            ray_setup(r, 0.0f);
+            float4 rec;
+            ray_cast(a.nodes, a.tris, a.hF, r, a.dist, &rec);
+            if (bvh_i(rec.y) >= 0 && (bvh_i(best.y) < 0 || rec.x < best.x)) { best = rec; side = s; }
+        }
+        const int32_t hf = bvh_i(best.y);
+        if (hf >= 0) {
+            off = side ? -best.x : best.x;
+            int32_t hv[3];
+            float hp[3][3], he1[3], he2[3], hg[3], N[3], t[3], b[3], n[3];
+            load_face(a.hpos, a.hfaces, hf, hv, hp, he1, he2, hg);
+            const float hw[3] = {PERF_FSUB_RN(PERF_FSUB_RN(1.0f, best.z), best.w), best.z, best.w};
+            shade_normal(a.hnormals, hv, hg, hw, N);
+            nt_frame(e1, e2, g, a.normals, v, a.uv + 6 * (int64_t)f, w, t, b, n);
+            uint8_t c[3];
+            if (nt_encode(t, b, n, N, c))
+                for (int k = 0; k < 3; ++k) out[k] = c[k];
+        }
+    }
+    for (int k = 0; k < 3; ++k) a.texel[3 * i + k] = out[k];
+    a.offset[i] = off;
 }
 
 // ---------------------------------------------------------------- kernels
@@ -476,7 +664,21 @@ __global__ void __launch_bounds__(128) mesh_cast_pano_kernel(const CastArgs a)
 __global__ void __launch_bounds__(128) mesh_shade_kernel(const ShadeArgs a)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.R) shade_ray(a, i);
+    if (i < a.R) shade_ray<false>(a, i);
+}
+
+__global__ void __launch_bounds__(128) mesh_shade_normal_texture_kernel(const ShadeArgs a)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.R) shade_ray<true>(a, i);
+}
+
+// One thread per texel in the atlas's Morton order: a warp holds neighbouring texels of one or two faces, whose rays are
+// parallel and start close together, so they traverse the same nodes.
+__global__ void __launch_bounds__(128) normal_texture_bake_kernel(const BakeArgs a)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.N) bake_texel(a, i);
 }
 
 // The product library launches the kernels; the test harness build runs the same bodies over host arrays.
@@ -609,26 +811,87 @@ int perf_mesh_cast_pano(const int32_t* d_nodes, const float* d_tris, uint64_t F,
     return PERF_OK;
 }
 
-int perf_mesh_shade(const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V, const int32_t* d_faces,
-                    uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv, const uint8_t* d_texture, int T,
-                    float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back, void* stream)
+static int shade_fill(ShadeArgs& a, const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V,
+                      const int32_t* d_faces, uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv,
+                      const uint8_t* d_texture, int T, float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back)
 {
-    if (R == 0) return PERF_OK;
     PERF_CHECK_ARG(V < (1ull << 31) && F < (1ull << 30), "mesh of %llu vertices / %llu faces: needs V < 2^31 and F < 2^30",
                    (unsigned long long)V, (unsigned long long)F);
     PERF_CHECK_ARG(d_hits && d_rays_d && d_rgb && d_distance && d_opacity && d_normal && d_back, "NULL pointer");
     PERF_CHECK_ARG(F == 0 || (d_vertices && d_faces), "NULL vertices or faces");
     PERF_CHECK_ARG(!d_texture || (d_uv && T > 0 && T <= 65536), "texture without uv or of side %d", T);
-    ShadeArgs a;
     memset(&a, 0, sizeof(a));
     a.hits = (const float4*)d_hits; a.R = (int64_t)R; a.d = d_rays_d; a.pos = d_vertices; a.V = (int64_t)V; a.faces = d_faces;
     a.F = (int64_t)F; a.colors = d_colors; a.normals = d_normals; a.uv = d_uv; a.texture = d_texture; a.T = T;
     a.rgb = d_rgb; a.dist = d_distance; a.op = d_opacity; a.nrm = d_normal; a.back = d_back;
+    return PERF_OK;
+}
+
+int perf_mesh_shade(const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V, const int32_t* d_faces,
+                    uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv, const uint8_t* d_texture, int T,
+                    float* d_rgb, float* d_distance, float* d_opacity, float* d_normal, uint8_t* d_back, void* stream)
+{
+    if (R == 0) return PERF_OK;
+    ShadeArgs a;
+    int rc = shade_fill(a, d_hits, d_rays_d, R, d_vertices, V, d_faces, F, d_colors, d_normals, d_uv, d_texture, T, d_rgb, d_distance,
+                        d_opacity, d_normal, d_back);
+    if (rc) return rc;
 #ifdef PERF_HOST_HARNESS
     (void)stream;
-    for (int64_t i = 0; i < a.R; ++i) shade_ray(a, i);
+    for (int64_t i = 0; i < a.R; ++i) shade_ray<false>(a, i);
 #else
     mesh_shade_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a);
+    PERF_LAUNCH_CHECK();
+#endif
+    return PERF_OK;
+}
+
+int perf_mesh_shade_normal_texture(const void* d_hits, const float* d_rays_d, uint64_t R, const float* d_vertices, uint64_t V,
+                                   const int32_t* d_faces, uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv,
+                                   const uint8_t* d_texture, const uint8_t* d_normal_texture, int T, float* d_rgb, float* d_distance,
+                                   float* d_opacity, float* d_normal, uint8_t* d_back, void* stream)
+{
+    if (R == 0) return PERF_OK;
+    PERF_CHECK_ARG(d_normal_texture && d_uv && T > 0 && T <= 65536, "normal texture without uv or of side %d", T);
+    ShadeArgs a;
+    int rc = shade_fill(a, d_hits, d_rays_d, R, d_vertices, V, d_faces, F, d_colors, d_normals, d_uv, d_texture, T, d_rgb, d_distance,
+                        d_opacity, d_normal, d_back);
+    if (rc) return rc;
+    a.ntex = d_normal_texture;
+#ifdef PERF_HOST_HARNESS
+    (void)stream;
+    for (int64_t i = 0; i < a.R; ++i) shade_ray<true>(a, i);
+#else
+    mesh_shade_normal_texture_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a);
+    PERF_LAUNCH_CHECK();
+#endif
+    return PERF_OK;
+}
+
+int perf_normal_texture_bake(const int32_t* d_nodes, const float* d_tris, const float* d_hi_vertices, uint64_t hi_V,
+                             const int32_t* d_hi_faces, uint64_t hi_F, const float* d_hi_normals, const float* d_vertices, uint64_t V,
+                             const int32_t* d_faces, uint64_t F, const float* d_normals, const float* d_uv, const int32_t* d_face,
+                             const float* d_point, uint64_t N, float distance, uint8_t* d_texel, float* d_offset, void* stream)
+{
+    if (N == 0) return PERF_OK;
+    PERF_CHECK_ARG(hi_V < (1ull << 31) && hi_F < (1ull << 30) && V < (1ull << 31) && F < (1ull << 30),
+                   "meshes of %llu / %llu vertices and %llu / %llu faces: need V < 2^31 and F < 2^30", (unsigned long long)hi_V,
+                   (unsigned long long)V, (unsigned long long)hi_F, (unsigned long long)F);
+    PERF_CHECK_ARG(N < (1ull << 40), "%llu texels", (unsigned long long)N);
+    PERF_CHECK_ARG(hi_F == 0 || (d_tris && (hi_F == 1 || d_nodes) && d_hi_vertices && d_hi_faces), "NULL high mesh or BVH");
+    PERF_CHECK_ARG(F == 0 || (d_vertices && d_faces && d_uv), "NULL low mesh or uv");
+    PERF_CHECK_ARG(d_face && d_point && d_texel && d_offset, "NULL pointer");
+    PERF_CHECK_ARG(distance >= 0.0f && distance < INFINITY, "cast distance %g: needs a finite distance >= 0", (double)distance);
+    BakeArgs a;
+    memset(&a, 0, sizeof(a));
+    a.nodes = d_nodes; a.tris = d_tris; a.hF = (int64_t)hi_F; a.hpos = d_hi_vertices; a.hfaces = d_hi_faces; a.hnormals = d_hi_normals;
+    a.pos = d_vertices; a.faces = d_faces; a.normals = d_normals; a.uv = d_uv; a.face = d_face; a.point = d_point; a.N = (int64_t)N;
+    a.dist = distance; a.texel = d_texel; a.offset = d_offset;
+#ifdef PERF_HOST_HARNESS
+    (void)stream;
+    for (int64_t i = 0; i < a.N; ++i) bake_texel(a, i);
+#else
+    normal_texture_bake_kernel<<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a);
     PERF_LAUNCH_CHECK();
 #endif
     return PERF_OK;

@@ -20,12 +20,16 @@ from .config import PERF_GRID
 # nerf.py:147-168), but on a fitted box room that level set is a cloud around the walls; 50 puts the vertices inside the
 # room on its walls and covers all of them (DESIGN.md section 6, tests/test_gpu_mesh.py::test_fitted_box_room_mesh).
 DEFAULT_THRESHOLD = 50.0
+# How far (voxels of the extraction lattice) the normal texture bake searches for the full-resolution surface on either side
+# of the decimated one
+NORMAL_TEXTURE_DISTANCE = 4.0
 
 
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
                  normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None,
-                 min_component: Optional[float] = None, max_cut: Optional[float] = None, texture_views=None) -> dict:
+                 min_component: Optional[float] = None, max_cut: Optional[float] = None, texture_views=None,
+                 normal_texture: bool = False, normal_texture_distance: float = NORMAL_TEXTURE_DISTANCE) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -39,24 +43,40 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     ``min_component`` and ``max_cut`` remove a fit's topological noise, both in voxels of the lattice (the smallest of
     extent / (r - 1) over the axes): components whose bounding-box diagonal is below ``min_component`` are dropped (floaters),
     and with ``target_faces`` the decimation cuts the mesh along non-face 3-cycles of perimeter <= ``max_cut`` where it would
-    otherwise stall (short handles through the walls); ``ops.decimate`` states both.  ``max_cut`` needs ``target_faces``."""
+    otherwise stall (short handles through the walls); ``ops.decimate`` states both.  ``max_cut`` needs ``target_faces``.
+    ``normal_texture`` keeps the detail the decimation removes as a tangent-space normal texture in the same atlas
+    (:func:`bake_normal_texture`, ``"normal_texture"`` and ``"normal_texture_hit_share"`` join the dict): its source is the
+    marching-tets mesh (after the floater removal when ``min_component`` is set) with the density-gradient normals, searched
+    within ``normal_texture_distance`` voxels of the decimated surface.  It needs ``target_faces`` and ``texture_size``; the
+    other outputs are the same with and without it."""
     if max_cut is not None and target_faces is None:
         raise ValueError("extract_mesh: max_cut acts on the decimation: it needs target_faces")
     if texture_views is not None and texture_size is None:
         raise ValueError("extract_mesh: texture_views colours the texture atlas: it needs texture_size")
+    if normal_texture and (target_faces is None or texture_size is None):
+        raise ValueError("extract_mesh: normal_texture bakes the full mesh into the decimated mesh's atlas: it needs target_faces "
+                         "and texture_size")
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     sigma = ops.fields_lattice(packed, geo_half, app_half, resolution, aabb, PERF_GRID)
     verts, faces = ops.marching_tets(sigma, threshold, aabb)
     del sigma
+    r3 = [int(resolution)] * 3 if isinstance(resolution, int) else [int(r) for r in resolution]
+    voxel = min((aabb[3 + d] - aabb[d]) / (r3[d] - 1) for d in range(3))
+    mc = None if min_component is None else float(min_component) * voxel
+    source, dropped = None, False
+    if normal_texture:
+        # the source is the mesh the decimation starts from: after the floater removal, which the decimation then skips
+        if mc is not None:
+            verts, faces = ops.drop_components(verts, faces, mc)
+            dropped = True
+        source = {"vertices": verts, "faces": faces,
+                  "normals": ops.fields_points(packed, geo_half, app_half, verts, aabb, PERF_GRID, normals=True)[2]}
     if min_component is not None or max_cut is not None:
-        r3 = [int(resolution)] * 3 if isinstance(resolution, int) else [int(r) for r in resolution]
-        voxel = min((aabb[3 + d] - aabb[d]) / (r3[d] - 1) for d in range(3))
-        mc = None if min_component is None else float(min_component) * voxel
         cut = None if max_cut is None else float(max_cut) * voxel
         if target_faces is not None:
-            verts, faces = ops.decimate(verts, faces, target_faces, max_cut=cut, min_component=mc)
+            verts, faces = ops.decimate(verts, faces, target_faces, max_cut=cut, min_component=mc, dropped=dropped)
         else:
             verts, faces = ops.drop_components(verts, faces, mc)
     elif target_faces is not None:
@@ -69,7 +89,11 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
         if normals:
             out["normals"] = res[2]
     if texture_size is not None:
-        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views))
+        # the low mesh's frame is built from the normals the mesh is returned with (the geometric normals without them), so
+        # every renderer of the result decodes the texture in the frame it was encoded in
+        nt = None if source is None else dict(source=source, normals=out.get("normals"), distance=float(normal_texture_distance) * voxel)
+        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views, normal=nt))
+        del nt, source                  # the full-resolution mesh and its normals (the BVH went with _bake)
     return out
 
 
@@ -81,30 +105,57 @@ TEXEL_CHUNK = 1 << 24       # texels per perf_atlas_texels / perf_fields_points 
 
 
 def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK, views=None,
-          depth_tol: float = ops.VIEWS_DEPTH_TOL) -> dict:
-    atlas = ops.texture_atlas(verts, faces, size)
+          depth_tol: float = ops.VIEWS_DEPTH_TOL, normal: Optional[dict] = None, atlas: Optional[dict] = None) -> dict:
+    """One walk over the atlas's texels in chunks: the colour field's texture (``packed`` not None), coloured from ``views``
+    where they see the texel, and the normal texture of ``normal`` = {"source": the high mesh, "normals": the low mesh's vertex
+    normals or None, "distance": world units} (:func:`bake_normal_texture`)."""
+    atlas = ops.texture_atlas(verts, faces, size) if atlas is None else atlas
     T = atlas["size"]
-    image = torch.zeros(T * T, 3, dtype=torch.uint8, device=verts.device)
+    dev = verts.device
+    if packed is not None:
+        image = torch.zeros(T * T, 3, dtype=torch.uint8, device=dev)
     if views is not None:
-        views = _packed_views(views, verts.device)
+        views = _packed_views(views, dev)
         fnormal = ops.face_normals(verts, faces)
-        view_img = torch.full((T * T,), -2, dtype=torch.int32, device=verts.device)
+        view_img = torch.full((T * T,), -2, dtype=torch.int32, device=dev)
+    if normal is not None:
+        src = normal["source"]
+        bvh = ops.mesh_bvh(src["vertices"], src["faces"])
+        nimage = torch.tensor([128, 128, 255], dtype=torch.uint8, device=dev).repeat(T * T, 1)
+        n_used = torch.zeros((), dtype=torch.int64, device=dev)
+        n_hit = torch.zeros((), dtype=torch.int64, device=dev)
     for m0 in range(0, atlas["used"], chunk):
         n = min(chunk, atlas["used"] - m0)
         face, point = ops.atlas_texels(verts, faces, atlas, m0, n)
-        rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
-        rgb[face < 0] = 0
-        x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=verts.device))
-        if views is not None:
-            vrgb, weight, view = ops.texture_views(point, face, fnormal, views, depth_tol)
-            rgb = torch.where((weight > 0)[:, None], _rgb8(vrgb), rgb)
-            view_img[(T - 1 - y) * T + x] = view
-            del vrgb, weight, view
-        image[(T - 1 - y) * T + x] = rgb
-        del face, point, rgb, x, y
-    out = {"uv": atlas["uv"], "texture": image.view(T, T, 3)}
+        x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=dev))
+        if packed is not None:
+            rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
+            rgb[face < 0] = 0
+            if views is not None:
+                vrgb, weight, view = ops.texture_views(point, face, fnormal, views, depth_tol)
+                rgb = torch.where((weight > 0)[:, None], _rgb8(vrgb), rgb)
+                view_img[(T - 1 - y) * T + x] = view
+                del vrgb, weight, view
+            image[(T - 1 - y) * T + x] = rgb
+            del rgb
+        if normal is not None:
+            texel, offset = ops.bake_normal_texture(bvh, src["vertices"], src["faces"], src.get("normals"), verts, faces,
+                                                    normal["normals"], atlas["uv"], face, point, normal["distance"])
+            nimage[(T - 1 - y) * T + x] = texel
+            n_used += (face >= 0).sum()
+            n_hit += torch.isfinite(offset).sum()
+            del texel, offset
+        del face, point, x, y
+    out = {"uv": atlas["uv"]}
+    if packed is not None:
+        out["texture"] = image.view(T, T, 3)
     if views is not None:
         out["texture_view"] = view_img.view(T, T)
+    if normal is not None:
+        out["normal_texture"] = nimage.view(T, T, 3)
+        used = int(n_used)
+        out["normal_texture_hit_share"] = int(n_hit) / used if used else 0.0
+        del bvh
     return out
 
 
@@ -132,6 +183,36 @@ def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size, views=views,
                               depth_tol=depth_tol))
+
+
+@torch.no_grad()
+def bake_normal_texture(mesh: dict, source: dict, distance: float, size: Optional[int] = None) -> dict:
+    """``mesh`` (a mesh with its atlas ``"uv"``: :func:`bake_texture` or :func:`extract_mesh` with ``texture_size``, or
+    :func:`read_obj`) with the detail of ``source`` -- the full-resolution surface it was decimated from, {"vertices",
+    "faces"[, "normals"]} -- baked into a tangent-space normal texture of the same atlas: adds ``"normal_texture"`` [T,T,3]
+    uint8 (row 0 at v = 1, the OpenGL / glTF convention: +G along +v) and ``"normal_texture_hit_share"``, the share of the
+    used texels whose casts hit ``source``.  T is ``size``, by default the side of the mesh's ``"texture"``.  Per texel,
+    rays from its point on the low surface along +/- its face's normal find the nearest ``source`` surface within
+    ``distance`` (world units); its shading normal (``source``'s vertex normals, else its face normal) is expressed in the
+    MikkTSpace frame of ``mesh`` (its vertex normals, else its face normals: the frame :func:`render_mesh` decodes in) and
+    stored as (c + 1) 127.5; texels with no hit are flat, (128, 128, 255).  The atlas layout is rebuilt (its texel points
+    need the per-face cell records the uv do not carry) and must reproduce the mesh's uv, else ValueError.
+    ``ops.bake_normal_texture`` and include/perfb200.h state the rule.  Needs no field."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    m = _on_gpu(mesh, dev)
+    if "uv" not in m:
+        raise ValueError("bake_normal_texture: the mesh needs its texture atlas uv")
+    if size is None:
+        if "texture" not in m:
+            raise ValueError("bake_normal_texture: pass the atlas side (size) for a mesh without a texture")
+        size = m["texture"].shape[0]
+    atlas = ops.texture_atlas(m["vertices"], m["faces"], int(size))
+    if not torch.equal(atlas["uv"], m["uv"]):
+        raise ValueError(f"bake_normal_texture: the mesh's uv are not the {size}^2 texture atlas of its faces")
+    src = _on_gpu(source, dev)
+    normal = {"source": src, "normals": m.get("normals"), "distance": float(distance)}
+    out = _bake(None, None, None, None, m["vertices"], m["faces"], int(size), normal=normal, atlas=atlas)
+    return dict(mesh, normal_texture=out["normal_texture"], normal_texture_hit_share=out["normal_texture_hit_share"])
 
 
 _PLY_PROPS = {"vertices": ("x", "y", "z"), "normals": ("nx", "ny", "nz"), "colors": ("red", "green", "blue")}
@@ -204,8 +285,9 @@ def _lines(fmt: str, a: np.ndarray) -> str:
 def write_obj(path: str, mesh: dict) -> None:
     """Wavefront OBJ of a textured mesh (a :func:`bake_texture` result): ``path`` with ``v`` (and ``vn`` when the mesh has
     normals), three ``vt`` per face (face f's corners are vt 3f + 1 .. 3f + 3) and ``f v/vt[/vn]``; ``<stem>.mtl`` with one
-    material whose ``map_Kd`` is ``<stem>_albedo.png``, the texture (8-bit RGB).  Floats are written with 9 significant digits,
-    so fp32 values read back exactly."""
+    material whose ``map_Kd`` is ``<stem>_albedo.png``, the texture (8-bit RGB).  With ``"normal_texture"`` the material also
+    has ``norm <stem>_normal.png`` (the normal-map key of the MTL PBR extension), that texture in the same atlas.  Floats are
+    written with 9 significant digits, so fp32 values read back exactly."""
     import os
     import cv2
     obj, mtl, png = obj_paths(path)
@@ -229,15 +311,22 @@ def write_obj(path: str, mesh: dict) -> None:
         fh.write(_lines("vt %.9g %.9g\n", uv.astype(np.float64)))
         fh.write("usemtl albedo\n")
         fh.write(_lines(ffmt, idx.reshape(F, -1)))
+    ntex = mesh.get("normal_texture")
+    npng = os.path.splitext(path)[0] + "_normal.png"
     with open(mtl, "w") as fh:
         fh.write(f"newmtl albedo\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd {os.path.basename(png)}\n")
+        if ntex is not None:
+            fh.write(f"norm {os.path.basename(npng)}\n")
     if not cv2.imwrite(png, np.ascontiguousarray(tex[:, :, ::-1])):
         raise OSError(f"write_obj: could not write {png}")
+    if ntex is not None and not cv2.imwrite(npng, np.ascontiguousarray(np.ascontiguousarray(_np(ntex), np.uint8)[:, :, ::-1])):
+        raise OSError(f"write_obj: could not write {npng}")
 
 
 def read_obj(path: str) -> dict:
     """Reads what :func:`write_obj` writes (numpy arrays): vertices, faces, uv [F,3,2], normals when present, and texture
-    [T,T,3] RGB from the PNG the MTL's ``map_Kd`` names."""
+    [T,T,3] RGB from the PNG the MTL's ``map_Kd`` names, and ``normal_texture`` from the one its ``norm`` names when it has
+    that line."""
     import os
     import cv2
     v, vn, vt, fl, mtl = [], [], [], [], None
@@ -266,10 +355,15 @@ def read_obj(path: str) -> dict:
     if mtl is not None:
         base = os.path.dirname(path)
         with open(os.path.join(base, mtl)) as fh:
-            png = next(ln.split(None, 1)[1].strip() for ln in fh if ln.startswith("map_Kd"))
+            keys = {w[0]: w[1] for w in (ln.split(None, 1) for ln in fh) if len(w) == 2}
+        png = keys["map_Kd"].strip()
         out["mtl"], out["map_Kd"] = mtl, png
         img = cv2.imread(os.path.join(base, png), cv2.IMREAD_UNCHANGED)
         out["texture"] = np.ascontiguousarray(img[:, :, ::-1])
+        if "norm" in keys:
+            out["norm"] = keys["norm"].strip()
+            img = cv2.imread(os.path.join(base, out["norm"]), cv2.IMREAD_UNCHANGED)
+            out["normal_texture"] = np.ascontiguousarray(img[:, :, ::-1])
     return out
 
 
@@ -278,7 +372,7 @@ def _np(a) -> np.ndarray:
 
 
 _MESH_DTYPES = {"vertices": torch.float32, "faces": torch.int32, "colors": torch.uint8, "normals": torch.float32,
-                "uv": torch.float32, "texture": torch.uint8}
+                "uv": torch.float32, "texture": torch.uint8, "normal_texture": torch.uint8}
 
 
 def _on_gpu(mesh: dict, device) -> dict:
@@ -303,7 +397,8 @@ def render_mesh(mesh: dict, pose=None, H: Optional[int] = None, W: Optional[int]
     """Renders a triangle mesh by ray casting on the GPU (``ops.mesh_bvh`` / ``mesh_cast(_pano)`` / ``mesh_shade``): the same
     outputs as ``NeRFScene.render_pano`` / ``render`` -- {"rgb" [..., 3], "distance" [..., 1], "opacities" [..., 1], "normal"
     [..., 3]} with the eval renders' background rule -- plus "back" [..., 1] bool, true where the hit face is a back face.
-    ``mesh``: an :func:`extract_mesh` result (with or without texture) or what :func:`read_ply` / :func:`read_obj` return.  Either
+    ``mesh``: an :func:`extract_mesh` result (with or without texture; with its ``"normal_texture"`` when it has one) or what
+    :func:`read_ply` / :func:`read_obj` return.  Either
     ``pose`` with ``H``, ``W`` (an equirectangular panorama, rows [row0, row0 + rows)) or ``rays`` ((o, d) or an object with
     ``.o`` / ``.d``, [..., 3]).  Only hits with t in [near, far] count.  Pass the ``bvh`` of an earlier call (``ops.mesh_bvh``)
     to render more views of the same mesh without rebuilding it."""
@@ -323,7 +418,8 @@ def render_mesh(mesh: dict, pose=None, H: Optional[int] = None, W: Optional[int]
         o, d = (rays.o, rays.d) if hasattr(rays, "o") else rays
         o, d = o.to(dev, torch.float32).contiguous(), d.to(dev, torch.float32).contiguous()
         hits = ops.mesh_cast(bvh, o, d, near, far)
-    return ops.mesh_shade(hits, d, m["vertices"], m["faces"], m.get("colors"), m.get("normals"), m.get("uv"), m.get("texture"))
+    return ops.mesh_shade(hits, d, m["vertices"], m["faces"], m.get("colors"), m.get("normals"), m.get("uv"), m.get("texture"),
+                          m.get("normal_texture"))
 
 
 def _psnr(a: torch.Tensor, b: torch.Tensor) -> float:

@@ -819,7 +819,7 @@ def drop_components(vertices: torch.Tensor, faces: torch.Tensor, min_component: 
 
 
 def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, stats: Optional[list] = None,
-             max_cut: Optional[float] = None, min_component: Optional[float] = None):
+             max_cut: Optional[float] = None, min_component: Optional[float] = None, dropped: bool = False):
     """Quadric-error edge collapse of a closed, consistently oriented, edge-manifold mesh (vertices [V,3] fp32, faces [F,3]
     int32; ``marching_tets`` output is one) down to ``target_faces`` faces: rounds of independent collapses
     (``perf_decimate_*``; include/perfb200.h states the rules).  Returns (vertices [V',3], faces [F',3]) with F' = target - 1 or
@@ -831,11 +831,16 @@ def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, sta
     dropped before the first round and after every cut round; with ``max_cut``, when a round selects no collapse, one cut
     round cuts the mesh along independent non-face 3-cycles of perimeter <= ``max_cut`` and caps both sides (a handle is
     removed, or a piece split off), and the collapse rounds go on.  With either set, ``stats`` receives ("collapse" | "cut" |
-    "drop", count) per round: collapses, cuts, components dropped.  Without them the call is exactly the one above."""
+    "drop", count) per round: collapses, cuts, components dropped.  Without them the call is exactly the one above.
+    ``dropped``: the mesh is already :func:`drop_components` of this ``min_component``, so the drop before the first round
+    would remove nothing and is skipped (stats get ("drop", 0)); vertex quadrics sum their faces in ascending face index and
+    the drop keeps the faces' order, so the result is the one the undropped mesh gives."""
     _check_shapes("decimate", vertices, faces)
     if isinstance(target_faces, bool) or int(target_faces) != target_faces or target_faces < 0:
         raise ValueError(f"decimate: target_faces must be an int >= 0, got {target_faces!r}")
     max_cut, min_component = _check_length("max_cut", max_cut), _check_length("min_component", min_component)
+    if dropped and min_component is None:
+        raise ValueError("decimate: dropped says which min_component the mesh has been through: it needs min_component")
     vertices, faces = _prepare("decimate", vertices, faces)
     clean = max_cut is not None or min_component is not None
     V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
@@ -850,7 +855,9 @@ def decimate(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, sta
         _call(L.perf_decimate_quadrics, _p(pos), V, _p(faces), F, _p(adj), _p(off), _p(quad), _stream())
         first = True
         if min_component is not None:
-            pos, quad, faces, n = _drop_components(pos, quad, faces, min_component)
+            n = 0
+            if not dropped:
+                pos, quad, faces, n = _drop_components(pos, quad, faces, min_component)
             if n:
                 V, F, first = pos.shape[0], faces.shape[0], False
             if stats is not None:
@@ -1078,11 +1085,13 @@ def hit_fields(hits: torch.Tensor):
 
 
 def mesh_shade(hits: torch.Tensor, rays_d: torch.Tensor, vertices: torch.Tensor, faces: torch.Tensor, colors=None, normals=None,
-               uv=None, texture=None) -> dict:
+               uv=None, texture=None, normal_texture=None) -> dict:
     """The eval renders' outputs from hit records [..., 4] (``perf_mesh_shade``): {"rgb" [..., 3], "distance" [..., 1],
     "opacities" [..., 1], "normal" [..., 3], "back" [..., 1] bool} with the background rule of the field renders.  Colour:
     ``colors`` [V,3] uint8 blended, or a bilinear lookup of ``texture`` [T,T,3] uint8 at the blended ``uv`` [F,3,2]; normal:
-    ``normals`` [V,3] blended, else the geometric normal (include/perfb200.h)."""
+    ``normals`` [V,3] blended, else the geometric normal (include/perfb200.h).  ``normal_texture`` [T,T,3] uint8 (a
+    :func:`bake_normal_texture` image, needs ``uv``; of the texture's side when there is one) is then applied in the
+    MikkTSpace frame of the hit (``perf_mesh_shade_normal_texture``)."""
     shape = tuple(hits.shape[:-1])
     hits = _chk(hits, torch.int32, "hits")
     d = _chk(rays_d, torch.float32, "rays_d")
@@ -1099,6 +1108,14 @@ def mesh_shade(hits: torch.Tensor, rays_d: torch.Tensor, vertices: torch.Tensor,
         if texture.dim() != 3 or texture.shape[0] != texture.shape[1] or texture.shape[2] != 3:
             raise ValueError(f"mesh_shade: texture must be [T, T, 3], got {tuple(texture.shape)}")
         T = texture.shape[0]
+    if normal_texture is not None:
+        if uv is None:
+            raise ValueError("mesh_shade: a normal texture needs uv")
+        uv, normal_texture = _chk(uv, torch.float32, "uv"), _chk(normal_texture, torch.uint8, "normal_texture")
+        nt = tuple(normal_texture.shape)
+        if len(nt) != 3 or nt[0] != nt[1] or nt[2] != 3 or (T and nt[0] != T):
+            raise ValueError(f"mesh_shade: normal_texture must be [T, T, 3] of the texture's side, got {nt}")
+        T = nt[0]
     dev = hits.device
     R = hits.numel() // 4
     rgb = torch.empty(*shape, 3, dtype=torch.float32, device=dev)
@@ -1107,9 +1124,44 @@ def mesh_shade(hits: torch.Tensor, rays_d: torch.Tensor, vertices: torch.Tensor,
     nrm = torch.empty(*shape, 3, dtype=torch.float32, device=dev)
     back = torch.empty(*shape, 1, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
-        _call(_L().perf_mesh_shade, _p(hits), _p(d), R, _p(vertices), vertices.shape[0], _p(faces), faces.shape[0], _p(colors),
-              _p(normals), _p(uv), _p(texture), T, _p(rgb), _p(dist), _p(op), _p(nrm), _p(back), _stream())
+        if normal_texture is None:
+            _call(_L().perf_mesh_shade, _p(hits), _p(d), R, _p(vertices), vertices.shape[0], _p(faces), faces.shape[0], _p(colors),
+                  _p(normals), _p(uv), _p(texture), T, _p(rgb), _p(dist), _p(op), _p(nrm), _p(back), _stream())
+        else:
+            _call(_L().perf_mesh_shade_normal_texture, _p(hits), _p(d), R, _p(vertices), vertices.shape[0], _p(faces),
+                  faces.shape[0], _p(colors), _p(normals), _p(uv), _p(texture), _p(normal_texture), T, _p(rgb), _p(dist), _p(op),
+                  _p(nrm), _p(back), _stream())
     return {"rgb": rgb, "distance": dist, "opacities": op, "normal": nrm, "back": back.bool()}
+
+
+def bake_normal_texture(bvh_hi: dict, hi_vertices: torch.Tensor, hi_faces: torch.Tensor, hi_normals, vertices: torch.Tensor,
+                        faces: torch.Tensor, normals, uv: torch.Tensor, face: torch.Tensor, point: torch.Tensor, distance: float):
+    """Tangent-space normal texels of the low mesh (``vertices``, ``faces``, ``normals`` [V,3] or None, its atlas ``uv``
+    [F,3,2]) at the texels ``face`` [N] int32 / ``point`` [N,3] of :func:`atlas_texels`, from the high mesh (``hi_*``, its
+    :func:`mesh_bvh` ``bvh_hi``): per texel two casts from the point along +/- the low face's unit normal over [0,
+    ``distance``] (world units), the high mesh's shading normal at the nearer hit encoded in the low mesh's MikkTSpace frame
+    (``perf_normal_texture_bake``; include/perfb200.h states the rule).  Returns (texel [N,3] uint8, (128, 128, 255) where
+    nothing is hit; offset [N] fp32, the signed distance to the hit along the face normal, +inf where nothing is hit)."""
+    hi_vertices, hi_faces = _chk(hi_vertices, torch.float32, "hi_vertices"), _chk(hi_faces, torch.int32, "hi_faces")
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    hi_normals = None if hi_normals is None else _chk(hi_normals, torch.float32, "hi_normals")
+    normals = None if normals is None else _chk(normals, torch.float32, "normals")
+    uv = _chk(uv, torch.float32, "uv")
+    face, point = _chk(face, torch.int32, "face"), _chk(point, torch.float32, "point")
+    N, dev = face.shape[0], face.device
+    if tuple(point.shape) != (N, 3) or tuple(uv.shape) != (faces.shape[0], 3, 2) or bvh_hi["F"] != hi_faces.shape[0]:
+        raise ValueError(f"bake_normal_texture: point {tuple(point.shape)}, uv {tuple(uv.shape)}, face {tuple(face.shape)}, "
+                         f"BVH of {bvh_hi['F']} faces for {hi_faces.shape[0]}: needs [N,3], [F,3,2], [N] and the high mesh's BVH")
+    for name, n, v in (("hi_normals", hi_normals, hi_vertices), ("normals", normals, vertices)):
+        if n is not None and tuple(n.shape) != tuple(v.shape):
+            raise ValueError(f"bake_normal_texture: {name} {tuple(n.shape)} for vertices {tuple(v.shape)}")
+    texel = torch.empty(N, 3, dtype=torch.uint8, device=dev)
+    offset = torch.empty(N, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_normal_texture_bake, _p(bvh_hi["nodes"]), _p(bvh_hi["tris"]), _p(hi_vertices), hi_vertices.shape[0],
+              _p(hi_faces), hi_faces.shape[0], _p(hi_normals), _p(vertices), vertices.shape[0], _p(faces), faces.shape[0],
+              _p(normals), _p(uv), _p(face), _p(point), N, float(distance), _p(texel), _p(offset), _stream())
+    return texel, offset
 
 
 VIEWS_MAX = 64              # perf_texture_views carries the poses in its kernel arguments

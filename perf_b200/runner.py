@@ -212,7 +212,10 @@ class CoreRunner:
         sees take the panoramas' colour instead of the field's (``mesh.bake_texture``'s ``views``), and the OBJ set is written
         as ``<stem>_views.obj`` / ``.mtl`` / ``_views_albedo.png``; the PLY and its vertex colours stay the field's.  With
         ``mesh_min_component`` and / or ``mesh_max_cut`` (voxels; ``NeRFScene.extract_mesh``) floaters and short handles are
-        removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  With ``mesh_report: true`` the written mesh
+        removed and the stem gets ``_clean`` (``mesh_<res>_f<target>_clean.ply``).  With ``mesh_normal_texture: true`` (needs
+        ``mesh_texture_size`` and ``mesh_target_faces``) the full-resolution surface is baked into a normal texture of the
+        same atlas, searched within ``mesh_normal_texture_distance`` voxels (default ``mesh.NORMAL_TEXTURE_DISTANCE``), and
+        written as ``<OBJ stem>_normal.png`` with a ``norm`` line in the MTL.  With ``mesh_report: true`` the written mesh
         is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
         (path, mesh) on rank 0, else (None, None)."""
         from .mesh import write_obj, write_ply
@@ -231,6 +234,14 @@ class CoreRunner:
                                                        "max_cut": None if cut is None else float(cut)}
         if views:
             clean["texture_views"] = self.sup_pool
+        if bool(self.conf.get("mesh_normal_texture", False)):
+            if tex is None or target is None:
+                raise ValueError("mesh_normal_texture bakes into the decimated mesh's atlas: it needs mesh_texture_size and "
+                                 "mesh_target_faces")
+            clean["normal_texture"] = True
+            nd = self.conf.get("mesh_normal_texture_distance", None)
+            if nd is not None:
+                clean["normal_texture_distance"] = float(nd)
         self.set_eval()
         if tex is None:
             mesh = self.scene.extract_mesh(res, None if thr is None else float(thr), target_faces=target, **clean)
@@ -256,7 +267,8 @@ class CoreRunner:
         ``<stem>_report.json`` (per pose the pose and its numbers) and per pose ``<stem>_report_<i>.png``, mesh rgb | field
         rgb | colourised |distance difference| (where both hit).  With ``views`` (registered panoramas, the ones the texture
         was coloured from) the JSON also gets ``"views"``, ``mesh.compare_to_views`` per panorama, and
-        ``"views_texel_share"``, the share of the used texels that the panoramas coloured.  Returns the report."""
+        ``"views_texel_share"``, the share of the used texels that the panoramas coloured.  A mesh with a normal texture adds
+        ``"normal_texture_hit_share"``.  Returns the report."""
         import json
         from .mesh import compare_to_field, compare_to_views
         poses = [torch.eye(4)]
@@ -278,6 +290,8 @@ class CoreRunner:
             tv = mesh["texture_view"]
             used = int((tv != -2).sum())
             report["views_texel_share"] = int((tv >= 0).sum()) / used if used else 0.0
+        if "normal_texture_hit_share" in mesh:
+            report["normal_texture_hit_share"] = mesh["normal_texture_hit_share"]
         with open(stem + "_report.json", "w") as f:
             json.dump(report, f, indent=1)
         return report
