@@ -398,6 +398,88 @@ int perf_atlas_layout(const float* d_vertices, uint64_t V, const int32_t* d_face
 int perf_atlas_texels(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_face_rec,
                       const int32_t* d_cells, uint64_t C, uint64_t m0, uint64_t n, int32_t* d_face, float* d_point, void* stream);
 
+/* ---- chart texture atlas of a triangle mesh (ops.chart_atlas drives it; csrc/charts.cu).  Same texture as perf_atlas_*: T
+ * a power of two in [256, 16384], texel (x, y) covers [x, x + 1] x [y, y + 1], y up; a texel's image index is
+ * (T - 1 - y) T + x (row 0 at v = 1).  fp64 steps are one rounded operation each, in the order written; dot products are
+ * (a0 b0 + a1 b1) + a2 b2.  Integer atomics only (min / max / add), so the result does not depend on arrival order.
+ * Charts (rounds over the dual graph, the decimation's selection pattern):
+ *   Start: chart f = face f, S_f = (p1 - p0) x (p2 - p0) in fp64 from the fp32 positions (twice the area-weighted normal),
+ *   alpha_f = 0.  Axis n = S / |S|; a chart with S = 0 (zero-area faces only) has none.
+ *   Dual edges (caller): an undirected edge {u, w} whose directed halves u -> w and w -> u each appear exactly once among the
+ *   faces' half-edges (faces[f][k] -> faces[f][(k+1) % 3]); boundary and non-manifold edges are never crossed.  Listed in
+ *   ascending order of the face corner 3f + k of their u < w half; edges [E,2] = the charts of the two faces.
+ *   Merge of A and B: n_AB = normalise(S_A + S_B); alpha_AB = max over the parts X with S_X != 0 of alpha_X + ang(n_X . n_AB);
+ *   0 when S_A = S_B = 0; not allowed when S_A + S_B = 0 otherwise.  ang(x) = sqrt(1 - x) P(x) + 1e-7 (Abramowitz & Stegun
+ *   4.4.46, |error| <= 2e-8 on [0, 1], Horner from the top coefficient; x clamped to 1; x < 0 is not allowed).  The pad keeps
+ *   the bound conservative: every face normal of a chart lies within alpha of its axis.  Allowed iff alpha_AB <= max_angle
+ *   (radians, in (0, pi/2)).
+ *   Selection: key = fp32 bits of alpha_AB << 32 | edge id (INT64_MAX when not allowed); cmin[c] = atomicMin over the allowed
+ *   edges at c; an edge is selected iff key == cmin of both charts: a matching.  Merge: the lower chart id A absorbs B: S_A +=
+ *   S_B, alpha_A = alpha_AB.  The caller relabels faces and edges (B -> A), drops the edges inside a chart (order kept) and
+ *   stops when a round selects nothing.  Charts are then numbered 0 .. C - 1 in order of their lowest face.
+ * Frames: n as above ((0, 0, 1) without one); b1, b2 of Duff et al. 2017: s = +1 if n.z >= 0 else -1, q = -1 / (s + n.z),
+ *   b = (n.x n.y) q, b1 = (1 + ((s n.x) n.x) q, s b, -(s n.x)), b2 = (b, s + (n.y n.y) q, -n.y); b1 x b2 = n.  Vertex p of a
+ *   chart: X = p . b1, Y = p . b2, and for k = 0 .. 7 with (c, s) = (cos, sin)(k pi / 16) (the fp64 constants in charts.cu):
+ *   x = c X + s Y, y = c Y - s X.  Boxes per (chart, k): integer atomicMin / Max of the order-preserving int64 image of the
+ *   fp64 bits.  The chart takes the k of smallest (x1 - x0)(y1 - y0), the first on a tie; when h = y1 - y0 > w = x1 - x0 it
+ *   is turned by (x, y) -> (y, -x).  rot = k (+ 8 when turned), frame = (x0, y0, w, h) in the final coordinates.
+ * Packing at density d (texels per world unit, fp32): cells = max(1, ceil(fp64(ext d))) per axis (capped at 2^24), the
+ *   rectangle cells + 2g, g = 2.  The caller sorts the rectangles by (h desc, w desc, chart) and fills shelves of width T
+ *   greedily: next[i] = the largest j with prefix[j] - prefix[i] <= T (binary search over the width prefix sums), shelf k
+ *   starts at next^k(0) (binary lifting: level l of the table is next^(2^l)), its height is its first rectangle's.  They fit
+ *   when every rectangle is <= T wide and tall and the shelf heights sum to <= T.  d is the bisection over the fp32 bit
+ *   patterns of ops.texture_atlas.  Rectangle origin: (prefix[i] - prefix[start of its shelf], sum of the heights below).
+ * UV: per corner in fixed point, 1/256 texel: per axis q = clamp(floor((local d) 256 + 0.5), 0, 256 cells), local = the
+ *   corner's frame coordinate minus x0 / y0, U = 256 (origin + g) + q; uv = fp32(U) / fp32(256 T), exact.  Corners that share
+ *   a vertex and a chart get identical bits.
+ * Texels: texel centre P = (256 x + 128, 256 y + 128).  Face f's candidates are the texels with P in its fixed-point box
+ *   widened by 256 g.  Face f contains P when its fixed-point doubled area is > 0 and each edge function (edge k+1 -> k+2)
+ *   is > 0, or 0 on a top-left edge (dy < 0, or dy = 0 and dx < 0).  Otherwise d2 = the squared distance to the nearest of its
+ *   edges 0-1, 1-2, 2-0 (fp64: s = clamp((r . e) / (e . e), 0, 1), 0 when e . e = 0; d2 = |r - s e|^2; strictly nearer wins),
+ *   and f competes iff d2 <= (256 g)^2.  key = f when contained, else (fp32 bits of d2 + 1) << 32 | f; the texel takes the
+ *   minimum key (INT64_MAX: unused).  Chart rectangles are disjoint and carry the g margin, so one chart competes per texel;
+ *   since g > sqrt 2, every texel a bilinear lookup at a point of a face reads belongs to that face's chart.  inside[m] counts
+ *   the faces that contain P: a texel with two marks its chart as overlapping (the caller splits such charts into single
+ *   faces and lays out once more).  Texel point: contained -> b_k = fp32(w_k / area) (fp64 division), p = (p0 + b1 (p1 -
+ *   p0)) + b2 (p2 - p0); else p = p_k + fp32(s) (p_k+1 - p_k) for the nearest edge k, fp32 steps.
+ * F < 2^29 and V < 2^31, else PERF_EINVAL. */
+/* d_sums [F,3] fp64 and d_alpha [F] (zero) of the single-face charts. */
+int perf_chart_sums(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, double* d_sums, double* d_alpha, void* stream);
+/* d_key [E] and d_cmin (per chart id, caller-set INT64_MAX, atomicMin) of the dual edges d_edges [E,2]. */
+int perf_chart_edges(const int32_t* d_edges, uint64_t E, const double* d_sums, const double* d_alpha, double max_angle, int64_t* d_key,
+                     int64_t* d_cmin, void* stream);
+/* d_selected [E] uint8. */
+int perf_chart_select(const int32_t* d_edges, uint64_t E, const int64_t* d_key, const int64_t* d_cmin, uint8_t* d_selected, void* stream);
+/* Merges the n selected edges d_selected_ids: d_sums / d_alpha of the lower chart. */
+int perf_chart_merge(const int32_t* d_edges, const int64_t* d_selected_ids, uint64_t n, double* d_sums, double* d_alpha, void* stream);
+/* d_chart [F] in [0, C), d_sums [C,3]; d_box [C,8,4] int64 set by the caller to INT64_MAX, INT64_MIN, INT64_MAX, INT64_MIN;
+ * writes d_rot [C] and d_frame [C,4] fp64 (two launches). */
+int perf_chart_frames(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_chart, uint64_t C,
+                      const double* d_sums, int64_t* d_box, int32_t* d_rot, double* d_frame, void* stream);
+/* d_rect [C,4] int32: cells x, cells y, rectangle width, height at the density. */
+int perf_chart_rects(const double* d_frame, uint64_t C, float density, int32_t* d_rect, void* stream);
+/* n sorted rectangles: d_prefix [n + 1] int64 exclusive width prefix (prefix[n] = total), d_height [n]; every width <= size.
+ * d_lift [levels, n + 1] (2^levels > n); writes d_start [n] (n past the last shelf) and d_shelf_h [n] (0 there);
+ * levels + 1 launches. */
+int perf_chart_shelves(const int64_t* d_prefix, const int32_t* d_height, uint64_t n, int size, int32_t* d_lift, int levels,
+                       int32_t* d_start, int32_t* d_shelf_h, void* stream);
+/* d_shelf_y [n] int64 exclusive prefix of d_shelf_h, d_order [n] the chart at each sorted position; writes d_origin [C,2]. */
+int perf_chart_place(const int64_t* d_prefix, const int32_t* d_start, const int64_t* d_shelf_y, const int32_t* d_order, uint64_t n,
+                     int32_t* d_origin, void* stream);
+/* d_uvq [F,3,2] int32 fixed point and d_uv [F,3,2] fp32. */
+int perf_chart_uv(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_chart, uint64_t C,
+                  const double* d_sums, const int32_t* d_rot, const double* d_frame, const int32_t* d_rect, const int32_t* d_origin,
+                  float density, int size, int32_t* d_uvq, float* d_uv, void* stream);
+/* d_count [F] int64 candidate texels per face. */
+int perf_chart_count(const int32_t* d_uvq, uint64_t F, int size, int64_t* d_count, void* stream);
+/* d_offsets [F + 1] exclusive scan of the counts (d_offsets[F] = total).  d_key [T^2] int64 (caller-set INT64_MAX, atomicMin),
+ * d_inside [T^2] int32 (zeroed, atomicAdd), both in image order. */
+int perf_chart_raster(const int32_t* d_uvq, uint64_t F, int size, const int64_t* d_offsets, uint64_t total, int64_t* d_key,
+                      int32_t* d_inside, void* stream);
+/* The n used texels d_index [n] (image index) / d_face [n] (their key's face): d_point [n,3] fp32 world sample points. */
+int perf_chart_texels(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const int32_t* d_uvq, int size,
+                      const int32_t* d_index, const int32_t* d_face, uint64_t n, float* d_point, void* stream);
+
 /* ---- ray casting of a triangle mesh (ops.mesh_bvh / mesh_cast / mesh_shade drive it; csrc/raycast.cu).  d_vertices [V,3] fp32,
  * d_faces [F,3] int32 (any triangle soup; zero-area faces are never hit).  F < 2^30 and V < 2^31, else PERF_EINVAL.
  * BVH (Karras 2012 linear BVH, deterministic: two builds of one mesh are byte-identical):

@@ -102,6 +102,18 @@ SIGNATURES = {
     "perf_atlas_legs": (i32, [vp, u64, vp, u64, vp, vp]),
     "perf_atlas_layout": (i32, [vp, u64, vp, u64, i32, vp, P(i32), i32, vp, vp, vp, vp]),
     "perf_atlas_texels": (i32, [vp, u64, vp, u64, vp, vp, u64, u64, u64, vp, vp, vp]),
+    "perf_chart_sums": (i32, [vp, u64, vp, u64, vp, vp, vp]),
+    "perf_chart_edges": (i32, [vp, u64, vp, vp, C.c_double, vp, vp, vp]),
+    "perf_chart_select": (i32, [vp, u64, vp, vp, vp, vp]),
+    "perf_chart_merge": (i32, [vp, vp, u64, vp, vp, vp]),
+    "perf_chart_frames": (i32, [vp, u64, vp, u64, vp, u64, vp, vp, vp, vp, vp]),
+    "perf_chart_rects": (i32, [vp, u64, f32, vp, vp]),
+    "perf_chart_shelves": (i32, [vp, vp, u64, i32, vp, i32, vp, vp, vp]),
+    "perf_chart_place": (i32, [vp, vp, vp, vp, u64, vp, vp]),
+    "perf_chart_uv": (i32, [vp, u64, vp, u64, vp, u64, vp, vp, vp, vp, vp, f32, i32, vp, vp, vp]),
+    "perf_chart_count": (i32, [vp, u64, i32, vp, vp]),
+    "perf_chart_raster": (i32, [vp, u64, i32, vp, u64, vp, vp, vp]),
+    "perf_chart_texels": (i32, [vp, u64, vp, u64, vp, i32, vp, vp, u64, vp, vp]),
     "perf_bvh_codes": (i32, [vp, u64, vp, u64, P(f32), P(f32), vp, vp]),
     "perf_bvh_topology": (i32, [vp, u64, vp, vp, vp]),
     "perf_bvh_boxes": (i32, [vp, u64, vp, u64, vp, vp, vp, vp, vp, vp]),

@@ -23,13 +23,23 @@ DEFAULT_THRESHOLD = 50.0
 # How far (voxels of the extraction lattice) the normal texture bake searches for the full-resolution surface on either side
 # of the decimated one
 NORMAL_TEXTURE_DISTANCE = 4.0
+# Largest angle (degrees) between a face normal and its chart's axis in the chart atlas (ops.chart_atlas), chosen from the
+# sweep over {30, 45, 60, 75} in DESIGN.md section 6 (tools/bench_chart_atlas.py)
+CHART_MAX_ANGLE = 60.0
+ATLASES = ("faces", "charts")
+
+
+def _check_atlas(name: str, atlas) -> str:
+    if atlas not in ATLASES:
+        raise ValueError(f"{name}: atlas must be one of {ATLASES}, got {atlas!r}")
+    return atlas
 
 
 @torch.no_grad()
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
                  normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None,
                  min_component: Optional[float] = None, max_cut: Optional[float] = None, texture_views=None,
-                 normal_texture: bool = False, normal_texture_distance: float = NORMAL_TEXTURE_DISTANCE) -> dict:
+                 normal_texture: bool = False, normal_texture_distance: float = NORMAL_TEXTURE_DISTANCE, atlas: str = "faces") -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -48,7 +58,11 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     (:func:`bake_normal_texture`, ``"normal_texture"`` and ``"normal_texture_hit_share"`` join the dict): its source is the
     marching-tets mesh (after the floater removal when ``min_component`` is set) with the density-gradient normals, searched
     within ``normal_texture_distance`` voxels of the decimated surface.  It needs ``target_faces`` and ``texture_size``; the
-    other outputs are the same with and without it."""
+    other outputs are the same with and without it.  ``atlas``: the texture layout, "faces" (one chart per face) or "charts"
+    (near-planar charts, :func:`bake_texture`), which the normal texture does not take yet."""
+    _check_atlas("extract_mesh", atlas)
+    if atlas != "faces" and normal_texture:
+        raise ValueError("extract_mesh: the normal texture's frame is defined for the per-face atlas: normal_texture needs atlas='faces'")
     if max_cut is not None and target_faces is None:
         raise ValueError("extract_mesh: max_cut acts on the decimation: it needs target_faces")
     if texture_views is not None and texture_size is None:
@@ -92,7 +106,7 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
         # the low mesh's frame is built from the normals the mesh is returned with (the geometric normals without them), so
         # every renderer of the result decodes the texture in the frame it was encoded in
         nt = None if source is None else dict(source=source, normals=out.get("normals"), distance=float(normal_texture_distance) * voxel)
-        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views, normal=nt))
+        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views, normal=nt, layout=atlas))
         del nt, source                  # the full-resolution mesh and its normals (the BVH went with _bake)
     return out
 
@@ -105,11 +119,15 @@ TEXEL_CHUNK = 1 << 24       # texels per perf_atlas_texels / perf_fields_points 
 
 
 def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK, views=None,
-          depth_tol: float = ops.VIEWS_DEPTH_TOL, normal: Optional[dict] = None, atlas: Optional[dict] = None) -> dict:
+          depth_tol: float = ops.VIEWS_DEPTH_TOL, normal: Optional[dict] = None, atlas: Optional[dict] = None,
+          layout: str = "faces") -> dict:
     """One walk over the atlas's texels in chunks: the colour field's texture (``packed`` not None), coloured from ``views``
     where they see the texel, and the normal texture of ``normal`` = {"source": the high mesh, "normals": the low mesh's vertex
-    normals or None, "distance": world units} (:func:`bake_normal_texture`)."""
-    atlas = ops.texture_atlas(verts, faces, size) if atlas is None else atlas
+    normals or None, "distance": world units} (:func:`bake_normal_texture`).  ``layout``: "faces" (``ops.texture_atlas``,
+    texels in Morton order) or "charts" (``ops.chart_atlas``, the used texels in image order)."""
+    charts = layout == "charts"
+    if atlas is None:
+        atlas = ops.chart_atlas(verts, faces, size) if charts else ops.texture_atlas(verts, faces, size)
     T = atlas["size"]
     dev = verts.device
     if packed is not None:
@@ -126,27 +144,35 @@ def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int 
         n_hit = torch.zeros((), dtype=torch.int64, device=dev)
     for m0 in range(0, atlas["used"], chunk):
         n = min(chunk, atlas["used"] - m0)
-        face, point = ops.atlas_texels(verts, faces, atlas, m0, n)
-        x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=dev))
+        if charts:
+            face, point, where = ops.chart_texels(verts, faces, atlas, m0, n)
+            where = where.long()
+        else:
+            face, point = ops.atlas_texels(verts, faces, atlas, m0, n)
+            x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=dev))
+            where = (T - 1 - y) * T + x
+            del x, y
         if packed is not None:
             rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
             rgb[face < 0] = 0
             if views is not None:
                 vrgb, weight, view = ops.texture_views(point, face, fnormal, views, depth_tol)
                 rgb = torch.where((weight > 0)[:, None], _rgb8(vrgb), rgb)
-                view_img[(T - 1 - y) * T + x] = view
+                view_img[where] = view
                 del vrgb, weight, view
-            image[(T - 1 - y) * T + x] = rgb
+            image[where] = rgb
             del rgb
         if normal is not None:
             texel, offset = ops.bake_normal_texture(bvh, src["vertices"], src["faces"], src.get("normals"), verts, faces,
                                                     normal["normals"], atlas["uv"], face, point, normal["distance"])
-            nimage[(T - 1 - y) * T + x] = texel
+            nimage[where] = texel
             n_used += (face >= 0).sum()
             n_hit += torch.isfinite(offset).sum()
             del texel, offset
-        del face, point, x, y
+        del face, point, where
     out = {"uv": atlas["uv"]}
+    if charts:
+        out.update(uv_vertices=atlas["uv_vertices"], uv_faces=atlas["uv_faces"])
     if packed is not None:
         out["texture"] = image.view(T, T, 3)
     if views is not None:
@@ -164,7 +190,7 @@ def _packed_views(views, device) -> dict:
 
 
 @torch.no_grad()
-def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops.VIEWS_DEPTH_TOL) -> dict:
+def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops.VIEWS_DEPTH_TOL, atlas: str = "faces") -> dict:
     """``mesh`` (an :func:`extract_mesh` result) with its colour field baked into a ``size`` x ``size`` texture (a power of two
     in [256, 16384]): adds ``"uv"`` [F,3,2] fp32 (per face corner, v up) and ``"texture"`` [T,T,3] uint8 (row 0 at v = 1).  One
     right-isosceles chart per face, packed in Z-order (``ops.texture_atlas``); each texel holds round(clip(rgb, 0, 1) * 255)
@@ -177,12 +203,19 @@ def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops
     result).  A texel that some panorama sees -- within ``depth_tol`` of its distance map, at a face angle of cos >= 0.15 --
     then takes the panoramas' colour (``ops.texture_views``: the cos / dist^2 weighted blend of the views that see it) instead
     of the field's, through the same rounding; the others keep the field's colour.  ``"texture_view"`` [T,T] int32 joins the
-    dict: per texel the view of the largest weight, -1 where the field coloured it, -2 where the texel is unused."""
+    dict: per texel the view of the largest weight, -1 where the field coloured it, -2 where the texel is unused.
+    ``atlas="charts"`` lays the texture out as near-planar charts instead (``ops.chart_atlas``): faces merged while every
+    normal stays within ``CHART_MAX_ANGLE`` degrees of the chart's axis, each chart projected onto its plane at one density,
+    with a 2-texel gutter, shelf-packed.  Each used texel holds the colour at the point of its face nearest to the texel
+    centre, and a bilinear lookup at any point of a face reads only texels of that face's chart.  ``"uv_vertices"`` [U,2]
+    and ``"uv_faces"`` [F,3] (one uv per chart and vertex) join the dict.  The face budget does not apply; ValueError when
+    the charts do not fit."""
+    _check_atlas("bake_texture", atlas)
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size, views=views,
-                              depth_tol=depth_tol))
+                              depth_tol=depth_tol, layout=atlas))
 
 
 @torch.no_grad()
@@ -284,7 +317,8 @@ def _lines(fmt: str, a: np.ndarray) -> str:
 
 def write_obj(path: str, mesh: dict) -> None:
     """Wavefront OBJ of a textured mesh (a :func:`bake_texture` result): ``path`` with ``v`` (and ``vn`` when the mesh has
-    normals), three ``vt`` per face (face f's corners are vt 3f + 1 .. 3f + 3) and ``f v/vt[/vn]``; ``<stem>.mtl`` with one
+    normals), three ``vt`` per face (face f's corners are vt 3f + 1 .. 3f + 3) -- or, when the mesh has ``"uv_faces"`` (the
+    chart atlas), its welded table ``"uv_vertices"`` with ``uv_faces`` as the indices -- and ``f v/vt[/vn]``; ``<stem>.mtl`` with one
     material whose ``map_Kd`` is ``<stem>_albedo.png``, the texture (8-bit RGB).  With ``"normal_texture"`` the material also
     has ``norm <stem>_normal.png`` (the normal-map key of the MTL PBR extension), that texture in the same atlas.  Floats are
     written with 9 significant digits, so fp32 values read back exactly."""
@@ -293,12 +327,13 @@ def write_obj(path: str, mesh: dict) -> None:
     obj, mtl, png = obj_paths(path)
     v = np.ascontiguousarray(_np(mesh["vertices"]), np.float32)
     f = np.ascontiguousarray(_np(mesh["faces"]), np.int64).reshape(-1, 3)
-    uv = np.ascontiguousarray(_np(mesh["uv"]), np.float32).reshape(-1, 2)
+    welded = mesh.get("uv_faces") is not None
+    uv = np.ascontiguousarray(_np(mesh["uv_vertices" if welded else "uv"]), np.float32).reshape(-1, 2)
     tex = np.ascontiguousarray(_np(mesh["texture"]), np.uint8)
     nrm = mesh.get("normals")
     F = f.shape[0]
     vi = f + 1
-    ti = np.arange(1, 3 * F + 1, dtype=np.int64).reshape(F, 3)
+    ti = np.ascontiguousarray(_np(mesh["uv_faces"]), np.int64).reshape(F, 3) + 1 if welded else np.arange(1, 3 * F + 1, dtype=np.int64).reshape(F, 3)
     if nrm is not None:
         idx, ffmt = np.stack([vi, ti, vi], 2), "f %d/%d/%d %d/%d/%d %d/%d/%d\n"
     else:
@@ -324,7 +359,8 @@ def write_obj(path: str, mesh: dict) -> None:
 
 
 def read_obj(path: str) -> dict:
-    """Reads what :func:`write_obj` writes (numpy arrays): vertices, faces, uv [F,3,2], normals when present, and texture
+    """Reads what :func:`write_obj` writes (numpy arrays): vertices, faces, uv [F,3,2] (with ``uv_vertices`` [U,2] and
+    ``uv_faces`` [F,3] when the ``vt`` table is welded, not three per face in order), normals when present, and texture
     [T,T,3] RGB from the PNG the MTL's ``map_Kd`` names, and ``normal_texture`` from the one its ``norm`` names when it has
     that line."""
     import os
@@ -350,6 +386,8 @@ def read_obj(path: str) -> dict:
     vt = np.asarray(vt, np.float32).reshape(-1, 2)
     out = {"vertices": np.asarray(v, np.float32).reshape(-1, 3), "faces": (fa[:, :, 0] - 1).astype(np.int32),
            "uv": vt[fa[:, :, 1] - 1] if len(fa) else np.zeros((0, 3, 2), np.float32)}
+    if len(fa) and not (len(vt) == 3 * len(fa) and np.array_equal(fa[:, :, 1].reshape(-1), np.arange(1, 3 * len(fa) + 1))):
+        out["uv_vertices"], out["uv_faces"] = vt, (fa[:, :, 1] - 1).astype(np.int32)
     if vn:
         out["normals"] = np.asarray(vn, np.float32).reshape(-1, 3)
     if mtl is not None:

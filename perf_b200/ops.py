@@ -1013,6 +1013,236 @@ def atlas_texels(vertices: torch.Tensor, faces: torch.Tensor, atlas: dict, m0: i
     return face, point
 
 
+CHART_GUTTER = 2            # texels of margin on each side of a chart's rectangle (perfb200.h: g)
+CHART_FIX = 256             # chart uv fixed point: 1/256 texel
+_NO_KEY64 = 2 ** 63 - 1
+
+
+def _dual_edges(faces: torch.Tensor, V: int) -> torch.Tensor:
+    """[E,2] int32 face pairs across the edges whose two directed halves each appear exactly once, in ascending order of the
+    corner 3f + k of their u < w half."""
+    fl = faces.long()
+    u, w = fl.reshape(-1), fl[:, [1, 2, 0]].reshape(-1)
+    hk, rk = u * V + w, w * V + u
+    skeys, order = torch.sort(hk, stable=True)
+
+    def count(k):
+        return torch.searchsorted(skeys, k, right=True) - torch.searchsorted(skeys, k)
+
+    h = torch.nonzero((u < w) & (count(hk) == 1) & (count(rk) == 1)).view(-1)
+    partner = order[torch.searchsorted(skeys, rk[h])]
+    e = torch.stack([h // 3, partner // 3], 1).to(torch.int32)
+    return e[e[:, 0] != e[:, 1]].contiguous()
+
+
+def _chart_driver(run, vertices: torch.Tensor, faces: torch.Tensor, size: int, max_angle: float, marks: Optional[list] = None) -> dict:
+    """The chart atlas's stages (``perf_chart_*``; include/perfb200.h states the rules) with torch for the sorts, scans,
+    relabelling and compaction in between.  ``run(name, *args)`` calls the library entry point ``name`` (stream appended):
+    :func:`chart_atlas` passes the product library and CUDA tensors, tests/chart_harness.py the host build and CPU tensors.
+    ``marks``: a list that receives (stage, CUDA event) at the stage boundaries."""
+    V, F, T, dev = vertices.shape[0], faces.shape[0], size, vertices.device
+    i32, i64, f64 = torch.int32, torch.int64, torch.float64
+
+    def mark(name):
+        if marks is not None:
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            marks.append((name, ev))
+
+    mark("start")
+    # -- charts: rounds of independent merges over the dual graph
+    S = torch.empty(F, 3, dtype=f64, device=dev)
+    alpha = torch.empty(F, dtype=f64, device=dev)
+    run("perf_chart_sums", _p(vertices), V, _p(faces), F, _p(S), _p(alpha))
+    S0 = S.clone()
+    label = torch.arange(F, dtype=i32, device=dev)            # chart of each face: its lowest face
+    edges = _dual_edges(faces, V)
+    rounds = 0
+    while edges.shape[0]:
+        E = edges.shape[0]
+        key = torch.empty(E, dtype=i64, device=dev)
+        cmin = torch.full((F,), _NO_KEY64, dtype=i64, device=dev)
+        run("perf_chart_edges", _p(edges), E, _p(S), _p(alpha), float(max_angle), _p(key), _p(cmin))
+        sel = torch.empty(E, dtype=torch.uint8, device=dev)
+        run("perf_chart_select", _p(edges), E, _p(key), _p(cmin), _p(sel))
+        ids = torch.nonzero(sel).view(-1)                     # the round's host read
+        if ids.numel() == 0:
+            break
+        run("perf_chart_merge", _p(edges), _p(ids), ids.numel(), _p(S), _p(alpha))
+        pair = edges[ids].long()
+        into = torch.arange(F, dtype=i32, device=dev)
+        into[pair.max(1).values] = pair.min(1).values.to(i32)
+        label = into[label.long()]
+        edges = into[edges.long()]
+        edges = edges[edges[:, 0] != edges[:, 1]].contiguous()
+        rounds += 1
+        del key, cmin, sel, ids, pair, into
+    mark("charts")
+
+    def layout(label):
+        roots, chart = torch.unique(label, sorted=True, return_inverse=True)
+        chart, C = chart.to(i32).contiguous(), roots.numel()
+        return roots, chart, C
+
+    def place(chart, C, Sc):
+        box = torch.empty(C, 8, 4, dtype=i64, device=dev)
+        box[..., 0::2], box[..., 1::2] = _NO_KEY64, -2 ** 63
+        rot = torch.empty(C, dtype=i32, device=dev)
+        frame = torch.empty(C, 4, dtype=f64, device=dev)
+        run("perf_chart_frames", _p(vertices), V, _p(faces), F, _p(chart), C, _p(Sc), _p(box), _p(rot), _p(frame))
+        del box
+        mark("frames")
+        rect = torch.empty(C, 4, dtype=i32, device=dev)
+        ids = torch.arange(C, dtype=i64, device=dev)
+
+        def pack(d):
+            """(fits, order, prefix, start, shelf_h) of the shelf packing at density d."""
+            run("perf_chart_rects", _p(frame), C, d, _p(rect))
+            rw, rh = rect[:, 2].long(), rect[:, 3].long()
+            if C == 0:
+                return True, None
+            if int(torch.maximum(rw.max(), rh.max())) > T:
+                return False, None
+            order = torch.argsort(((T + 1 - rh) << 45) | ((T + 1 - rw) << 30) | ids)
+            prefix = torch.zeros(C + 1, dtype=i64, device=dev)
+            prefix[1:] = torch.cumsum(rw[order], 0)
+            height = rh[order].to(i32).contiguous()
+            levels = C.bit_length()
+            lift = torch.empty(levels, C + 1, dtype=i32, device=dev)
+            start = torch.empty(C, dtype=i32, device=dev)
+            shelf_h = torch.empty(C, dtype=i32, device=dev)
+            run("perf_chart_shelves", _p(prefix), _p(height), C, T, _p(lift), levels, _p(start), _p(shelf_h))
+            fits = int(shelf_h.sum(dtype=i64)) <= T
+            return fits, (order.to(i32).contiguous(), prefix, start, shelf_h)
+
+        if not pack(0.0)[0]:
+            need = next((t for t in (256 << j for j in range(7)) if _chart_fit_at_zero(C, t)), None)
+            raise ValueError(f"chart_atlas: {C} charts do not fit a {T}^2 texture even at the smallest chart size "
+                             f"({1 + 2 * CHART_GUTTER}x{1 + 2 * CHART_GUTTER} texels each); "
+                             + (f"a {need}^2 texture holds them" if need else "no texture up to 16384^2 holds them")
+                             + ": use a larger texture size, or decimate the mesh further")
+        lo, hi = 0, 0x7F800000 if C else 1                   # fp32 bits: fits(lo) holds, hi = +inf is never tried
+        while hi - lo > 1:
+            mid = (lo + hi) // 2
+            if pack(_f32_bits(mid))[0]:
+                lo = mid
+            else:
+                hi = mid
+        d = _f32_bits(lo)
+        if C:
+            order, prefix, start, shelf_h = pack(d)[1]
+        else:
+            order, start, shelf_h = (torch.empty(0, dtype=i32, device=dev) for _ in range(3))
+            prefix = torch.zeros(1, dtype=i64, device=dev)
+        mark("search")
+        shelf_y = torch.cumsum(shelf_h.long(), 0) - shelf_h.long()
+        origin = torch.empty(C, 2, dtype=i32, device=dev)
+        run("perf_chart_place", _p(prefix), _p(start), _p(shelf_y), _p(order), C, _p(origin))
+        uvq = torch.empty(F, 3, 2, dtype=i32, device=dev)
+        uv = torch.empty(F, 3, 2, dtype=torch.float32, device=dev)
+        run("perf_chart_uv", _p(vertices), V, _p(faces), F, _p(chart), C, _p(Sc), _p(rot), _p(frame), _p(rect), _p(origin), d, T,
+            _p(uvq), _p(uv))
+        count = torch.empty(F, dtype=i64, device=dev)
+        run("perf_chart_count", _p(uvq), F, T, _p(count))
+        offsets = torch.zeros(F + 1, dtype=i64, device=dev)
+        offsets[1:] = torch.cumsum(count, 0)
+        total = int(offsets[-1])
+        key = torch.full((T * T,), _NO_KEY64, dtype=i64, device=dev)
+        inside = torch.zeros(T * T, dtype=i32, device=dev)
+        run("perf_chart_raster", _p(uvq), F, T, _p(offsets), total, _p(key), _p(inside))
+        over = torch.unique(chart[(key[inside >= 2] & 0xFFFFFFFF)])
+        index = torch.nonzero(key != _NO_KEY64).view(-1)
+        face = (key[index] & 0xFFFFFFFF).to(i32)
+        mark("raster")
+        return {"uv": uv, "uvq": uvq, "density": d, "texel_index": index.to(i32), "texel_face": face, "overlapping": over}
+
+    roots, chart, C = layout(label)
+    out = place(chart, C, S[roots.long()].contiguous())
+    split = int(out["overlapping"].numel())
+    if split:
+        # overlapping charts become single-face charts; the second layout cannot overlap
+        alone = torch.isin(chart, out["overlapping"].to(i32))
+        label = torch.where(alone, torch.arange(F, dtype=i32, device=dev), roots.to(i32)[chart.long()])
+        del out
+        roots, chart, C = layout(label)
+        r = roots.long()
+        out = place(chart, C, torch.where(alone[r][:, None], S0[r], S[r]).contiguous())
+    ck = (chart.long()[:, None] * V + faces.long()).reshape(-1)
+    uniq, inv = torch.unique(ck, sorted=True, return_inverse=True)
+    uv_vertices = torch.empty(uniq.numel(), 2, dtype=torch.float32, device=dev)
+    uv_vertices[inv] = out["uv"].reshape(-1, 2)
+    out.update(uv_vertices=uv_vertices, uv_faces=inv.view(F, 3).to(i32), chart=chart, charts=C, size=T,
+               used=int(out["texel_index"].numel()), rounds=rounds, split=split)
+    return out
+
+
+def _chart_fit_at_zero(C: int, size: int) -> bool:
+    """Do C charts of the smallest rectangle (1 + 2g texels square) fit a size^2 texture?"""
+    s = 1 + 2 * CHART_GUTTER
+    per = size // s
+    return C == 0 or -(-C // per) * s <= size
+
+
+CHART_MAX_ANGLE_LIMIT = 90.0
+
+
+def chart_atlas(vertices: torch.Tensor, faces: torch.Tensor, size: int, max_angle: Optional[float] = None, marks: Optional[list] = None) -> dict:
+    """Chart texture atlas of a triangle mesh (vertices [V,3] fp32, faces [F,3] int32; any triangle soup, open or closed) on a
+    ``size`` x ``size`` texture (a power of two in [256, 16384]): the surface is cut into near-planar charts -- faces merged
+    across manifold edges in rounds while every face normal stays within ``max_angle`` degrees (default
+    ``mesh.CHART_MAX_ANGLE``) of the chart's axis -- each projected onto its plane at one density d (texels per world unit),
+    in the smallest of 8 rotated rectangles, with a 2-texel gutter, and the rectangles shelf-packed; charts that overlap
+    themselves in the projection are split into single faces (``perf_chart_*``; include/perfb200.h states the rules).
+    Deterministic: repeated runs are byte-identical.  Returns {"uv": [F,3,2] fp32 (v up), "uv_vertices": [U,2] fp32 and
+    "uv_faces": [F,3] int32 (the welded table: one entry per (chart, vertex)), "chart": [F] int32, "charts": C, "density": d,
+    "size": size, "used": texels the charts claim, "uvq": [F,3,2] int32 fixed-point uv (1/256 texel), "texel_index" /
+    "texel_face": [used] int32 image index (row 0 at v = 1) and face of each used texel, "rounds": merge rounds, "split":
+    charts split for overlapping}; :func:`chart_texels` takes it.  Raises ValueError when the charts do not fit even at the
+    smallest chart size."""
+    if isinstance(size, bool) or int(size) != size or not (256 <= size <= 16384) or size & (size - 1):
+        raise ValueError(f"chart_atlas: size must be a power of two in [256, 16384], got {size!r}")
+    if max_angle is None:
+        from .mesh import CHART_MAX_ANGLE
+        max_angle = CHART_MAX_ANGLE
+    if isinstance(max_angle, bool) or not isinstance(max_angle, (int, float)) or not (0.0 < max_angle < CHART_MAX_ANGLE_LIMIT):
+        raise ValueError(f"chart_atlas: max_angle must be in (0, 90) degrees, got {max_angle!r}")
+    _check_shapes("chart_atlas", vertices, faces)
+    vertices, faces = _prepare("chart_atlas", vertices, faces)
+    V, F, dev = vertices.shape[0], faces.shape[0], vertices.device
+    if F >= 2 ** 29:
+        raise ValueError(f"chart_atlas: {F} faces: needs F < 2^29")
+    L = _L()
+    with torch.cuda.device(dev):
+        if F:
+            lo_i, hi_i = (int(v) for v in torch.stack([faces.min(), faces.max()]).tolist())
+            if lo_i < 0 or hi_i >= V:
+                raise ValueError(f"chart_atlas: face indices span [{lo_i}, {hi_i}], outside [0, {V})")
+
+        def run(name, *args):
+            _call(getattr(L, name), *args, _stream(), launches=2 if name in ("perf_chart_frames",) else 1)
+
+        return _chart_driver(run, vertices, faces, int(size), math.radians(float(max_angle)), marks)
+
+
+def chart_texels(vertices: torch.Tensor, faces: torch.Tensor, atlas: dict, m0: int = 0, n: Optional[int] = None):
+    """Used texels [m0, m0 + n) (default: all) of ``atlas`` (:func:`chart_atlas` of this mesh), in image order: (face [n]
+    int32, point [n,3] fp32 world -- the point of the face nearest to the texel centre --, image index [n] int32, row 0 at
+    v = 1): ``perf_chart_texels``."""
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces")
+    used = atlas["used"]
+    n = used - m0 if n is None else int(n)
+    if m0 < 0 or n < 0 or m0 + n > used:
+        raise ValueError(f"chart_texels: range [{m0}, {m0 + n}) outside [0, {used})")
+    dev = vertices.device
+    face = atlas["texel_face"][m0:m0 + n].contiguous()
+    index = atlas["texel_index"][m0:m0 + n].contiguous()
+    point = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_chart_texels, _p(vertices), vertices.shape[0], _p(faces), faces.shape[0], _p(atlas["uvq"]), atlas["size"],
+              _p(index), _p(face), n, _p(point), _stream())
+    return face, point, index
+
+
 def mesh_bvh(vertices: torch.Tensor, faces: torch.Tensor) -> dict:
     """Linear BVH (Karras 2012) of a triangle mesh (vertices [V,3] fp32, faces [F,3] int32) for :func:`mesh_cast`: the code box
     (the exact vertex min / max), ``perf_bvh_codes``, a stable sort, ``perf_bvh_topology`` and ``perf_bvh_boxes``
