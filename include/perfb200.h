@@ -601,6 +601,28 @@ int perf_texture_views(const float* d_points, const int32_t* d_face, uint64_t N,
                        const float* d_views, int n_views, int H, int W, const float* h_poses, float depth_tol, float* d_rgb,
                        float* d_weight, int32_t* d_view, void* stream);
 
+/* ---- pull-push fill of a texture's unused texels (ops.texture_fill drives it; csrc/texture_fill.cu).  d_image [T,T,3]
+ * uint8 (rows in image order, row 0 at v = 1), d_used [T,T] uint8 (nonzero: used), T a power of two in [256, 16384];
+ * h_empty 3 host bytes.  For each level l = 0 .. log2 T, block B_l(i, j) is the aligned square of texels [i 2^l, (i + 1) 2^l)
+ * x [j 2^l, (j + 1) 2^l) in image coordinates (T is a power of two, so flipping the rows keeps 2^l alignment); count is the
+ * number of used texels of the block and sum[c] the exact integer sum of channel c over them (int64: at 16384^2 the top sum
+ * reaches 6.8e10).
+ *   Output d_out [T,T,3]: a used texel is unchanged, byte for byte.  An unused texel p takes, per channel,
+ *   (2 sum + count) / (2 count) (integer division: the mean rounded half up) of the smallest block with l >= 1 that contains
+ *   p and has count > 0.  With no used texel at all, every texel is h_empty.
+ *   Guarantee: for every level l and every block with count > 0, every filled texel of the block lies per channel in [min,
+ *   max] of the block's used texels, so the box-filter mean over the block (a viewer's mip level l before its own rounding)
+ *   does too: a mip block never takes a colour from outside itself and black is never introduced.  Neighbouring charts that
+ *   share a block still mix: the fill does not make an atlas mip-safe between charts.  Base-level lookups that read only used
+ *   texels do not change.
+ * Integer arithmetic only, no atomics: the result does not depend on execution order.  d_out may be d_image (in place), no
+ * other overlap.  d_image, d_used, d_out and d_workspace 16-byte aligned; d_workspace of at least
+ * perf_texture_fill_workspace_bytes(T) bytes: 32 bytes per block of levels 5 .. log2 T, sum over l of (T >> l)^2 records, about
+ * 4/3 T^2 / 1024 (2.8 MB at 8192^2); its contents on entry do not matter. */
+uint64_t perf_texture_fill_workspace_bytes(int size);     /* 0 for a size outside the rule */
+int perf_texture_fill(const uint8_t* d_image, const uint8_t* d_used, int size, const uint8_t* h_empty, void* d_workspace,
+                      uint64_t workspace_bytes, uint8_t* d_out, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

@@ -123,6 +123,8 @@ SIGNATURES = {
     "perf_normal_texture_bake": (i32, [vp, vp, vp, u64, vp, u64, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, f32, vp, vp, vp]),
     "perf_mesh_shade_normal_texture": (i32, [vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]),
     "perf_texture_views": (i32, [vp, vp, u64, vp, u64, vp, i32, i32, i32, P(f32), f32, vp, vp, vp, vp]),
+    "perf_texture_fill_workspace_bytes": (u64, [i32]),
+    "perf_texture_fill": (i32, [vp, vp, i32, P(C.c_uint8), vp, u64, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),
     "perf_hashgrid_bwd_rays": (i32, [P(GridCfg), P(f32), vp, vp, vp, u64, u32, f32, f32, vp, vp, vp]),

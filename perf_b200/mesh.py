@@ -39,7 +39,8 @@ def _check_atlas(name: str, atlas) -> str:
 def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: float = DEFAULT_THRESHOLD, colors: bool = True,
                  normals: bool = True, target_faces: Optional[int] = None, texture_size: Optional[int] = None,
                  min_component: Optional[float] = None, max_cut: Optional[float] = None, texture_views=None,
-                 normal_texture: bool = False, normal_texture_distance: float = NORMAL_TEXTURE_DISTANCE, atlas: str = "faces") -> dict:
+                 normal_texture: bool = False, normal_texture_distance: float = NORMAL_TEXTURE_DISTANCE, atlas: str = "faces",
+                 texture_fill: bool = False) -> dict:
     """Mesh of the surface {sigma = threshold} of ``nerf`` (an ``NGPNeRF``), extracted on a lattice of ``resolution`` nodes per
     axis (an int or (rx, ry, rz)) spanning ``nerf.aabb``, faces included; the field is 0 on the box faces, so every surface
     closes there.  Returns ``{"vertices": [V,3] f32 world, "faces": [F,3] int32}`` (triangles facing free space, away from high
@@ -59,7 +60,8 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
     marching-tets mesh (after the floater removal when ``min_component`` is set) with the density-gradient normals, searched
     within ``normal_texture_distance`` voxels of the decimated surface.  It needs ``target_faces`` and ``texture_size``; the
     other outputs are the same with and without it.  ``atlas``: the texture layout, "faces" (one chart per face) or "charts"
-    (near-planar charts, :func:`bake_texture`), which the normal texture does not take yet."""
+    (near-planar charts, :func:`bake_texture`), which the normal texture does not take yet.  ``texture_fill`` fills the
+    unused texels of the textures (:func:`bake_texture`'s ``fill``); it needs ``texture_size``."""
     _check_atlas("extract_mesh", atlas)
     if atlas != "faces" and normal_texture:
         raise ValueError("extract_mesh: the normal texture's frame is defined for the per-face atlas: normal_texture needs atlas='faces'")
@@ -67,6 +69,8 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
         raise ValueError("extract_mesh: max_cut acts on the decimation: it needs target_faces")
     if texture_views is not None and texture_size is None:
         raise ValueError("extract_mesh: texture_views colours the texture atlas: it needs texture_size")
+    if texture_fill and texture_size is None:
+        raise ValueError("extract_mesh: texture_fill fills the texture atlas's unused texels: it needs texture_size")
     if normal_texture and (target_faces is None or texture_size is None):
         raise ValueError("extract_mesh: normal_texture bakes the full mesh into the decimated mesh's atlas: it needs target_faces "
                          "and texture_size")
@@ -106,7 +110,8 @@ def extract_mesh(nerf, resolution: Union[int, Sequence[int]] = 512, threshold: f
         # the low mesh's frame is built from the normals the mesh is returned with (the geometric normals without them), so
         # every renderer of the result decodes the texture in the frame it was encoded in
         nt = None if source is None else dict(source=source, normals=out.get("normals"), distance=float(normal_texture_distance) * voxel)
-        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views, normal=nt, layout=atlas))
+        out.update(_bake(packed, geo_half, app_half, aabb, verts, faces, texture_size, views=texture_views, normal=nt, layout=atlas,
+                         fill=texture_fill))
         del nt, source                  # the full-resolution mesh and its normals (the BVH went with _bake)
     return out
 
@@ -120,11 +125,13 @@ TEXEL_CHUNK = 1 << 24       # texels per perf_atlas_texels / perf_fields_points 
 
 def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int = TEXEL_CHUNK, views=None,
           depth_tol: float = ops.VIEWS_DEPTH_TOL, normal: Optional[dict] = None, atlas: Optional[dict] = None,
-          layout: str = "faces") -> dict:
+          layout: str = "faces", fill: bool = False) -> dict:
     """One walk over the atlas's texels in chunks: the colour field's texture (``packed`` not None), coloured from ``views``
     where they see the texel, and the normal texture of ``normal`` = {"source": the high mesh, "normals": the low mesh's vertex
     normals or None, "distance": world units} (:func:`bake_normal_texture`).  ``layout``: "faces" (``ops.texture_atlas``,
-    texels in Morton order) or "charts" (``ops.chart_atlas``, the used texels in image order)."""
+    texels in Morton order) or "charts" (``ops.chart_atlas``, the used texels in image order).  ``fill``: the textures' unused
+    texels are then filled (``ops.texture_fill``) from (0, 0, 0) for the albedo and the flat (128, 128, 255) for the normal
+    texture when no texel is used."""
     charts = layout == "charts"
     if atlas is None:
         atlas = ops.chart_atlas(verts, faces, size) if charts else ops.texture_atlas(verts, faces, size)
@@ -142,6 +149,8 @@ def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int 
         nimage = torch.tensor([128, 128, 255], dtype=torch.uint8, device=dev).repeat(T * T, 1)
         n_used = torch.zeros((), dtype=torch.int64, device=dev)
         n_hit = torch.zeros((), dtype=torch.int64, device=dev)
+    if fill:
+        used = torch.zeros(T * T, dtype=torch.bool, device=dev)
     for m0 in range(0, atlas["used"], chunk):
         n = min(chunk, atlas["used"] - m0)
         if charts:
@@ -152,6 +161,8 @@ def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int 
             x, y = ops.morton_xy(torch.arange(m0, m0 + n, dtype=torch.int64, device=dev))
             where = (T - 1 - y) * T + x
             del x, y
+        if fill:
+            used[where] = face >= 0
         if packed is not None:
             rgb = _rgb8(ops.fields_points(packed, geo_half, app_half, point, aabb, PERF_GRID)[1])
             rgb[face < 0] = 0
@@ -174,11 +185,11 @@ def _bake(packed, geo_half, app_half, aabb, verts, faces, size: int, chunk: int 
     if charts:
         out.update(uv_vertices=atlas["uv_vertices"], uv_faces=atlas["uv_faces"])
     if packed is not None:
-        out["texture"] = image.view(T, T, 3)
+        out["texture"] = ops.texture_fill(image.view(T, T, 3), used.view(T, T)) if fill else image.view(T, T, 3)
     if views is not None:
         out["texture_view"] = view_img.view(T, T)
     if normal is not None:
-        out["normal_texture"] = nimage.view(T, T, 3)
+        out["normal_texture"] = ops.texture_fill(nimage.view(T, T, 3), used.view(T, T), (128, 128, 255)) if fill else nimage.view(T, T, 3)
         used = int(n_used)
         out["normal_texture_hit_share"] = int(n_hit) / used if used else 0.0
         del bvh
@@ -190,7 +201,8 @@ def _packed_views(views, device) -> dict:
 
 
 @torch.no_grad()
-def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops.VIEWS_DEPTH_TOL, atlas: str = "faces") -> dict:
+def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops.VIEWS_DEPTH_TOL, atlas: str = "faces",
+                 fill: bool = False) -> dict:
     """``mesh`` (an :func:`extract_mesh` result) with its colour field baked into a ``size`` x ``size`` texture (a power of two
     in [256, 16384]): adds ``"uv"`` [F,3,2] fp32 (per face corner, v up) and ``"texture"`` [T,T,3] uint8 (row 0 at v = 1).  One
     right-isosceles chart per face, packed in Z-order (``ops.texture_atlas``); each texel holds round(clip(rgb, 0, 1) * 255)
@@ -209,17 +221,22 @@ def bake_texture(nerf, mesh: dict, size: int, views=None, depth_tol: float = ops
     with a 2-texel gutter, shelf-packed.  Each used texel holds the colour at the point of its face nearest to the texel
     centre, and a bilinear lookup at any point of a face reads only texels of that face's chart.  ``"uv_vertices"`` [U,2]
     and ``"uv_faces"`` [F,3] (one uv per chart and vertex) join the dict.  The face budget does not apply; ValueError when
-    the charts do not fit."""
+    the charts do not fit.
+    ``fill``: every texel no face claims (black otherwise) takes the rounded mean of the used texels of the smallest aligned
+    2^l x 2^l block (l >= 1) around it that has any (``ops.texture_fill``, pull-push).  The used texels, and so every
+    base-level lookup on the mesh, are unchanged, and each block of each level of a box-filtered mip chain keeps within the
+    colour range of its used texels, so mipmaps a viewer builds no longer darken towards the gutters.  Charts that share a
+    block still mix there.  ``"texture_view"`` still marks unused texels -2."""
     _check_atlas("bake_texture", atlas)
     aabb = [float(v) for v in nerf.aabb.tolist()]
     geo_half, app_half = nerf.geo_mlp._half(), nerf.app_mlp._half()
     packed = ops.pack_tables(geo_half, app_half, PERF_GRID)
     return dict(mesh, **_bake(packed, geo_half, app_half, aabb, mesh["vertices"], mesh["faces"], size, views=views,
-                              depth_tol=depth_tol, layout=atlas))
+                              depth_tol=depth_tol, layout=atlas, fill=fill))
 
 
 @torch.no_grad()
-def bake_normal_texture(mesh: dict, source: dict, distance: float, size: Optional[int] = None) -> dict:
+def bake_normal_texture(mesh: dict, source: dict, distance: float, size: Optional[int] = None, fill: bool = False) -> dict:
     """``mesh`` (a mesh with its atlas ``"uv"``: :func:`bake_texture` or :func:`extract_mesh` with ``texture_size``, or
     :func:`read_obj`) with the detail of ``source`` -- the full-resolution surface it was decimated from, {"vertices",
     "faces"[, "normals"]} -- baked into a tangent-space normal texture of the same atlas: adds ``"normal_texture"`` [T,T,3]
@@ -230,7 +247,9 @@ def bake_normal_texture(mesh: dict, source: dict, distance: float, size: Optiona
     MikkTSpace frame of ``mesh`` (its vertex normals, else its face normals: the frame :func:`render_mesh` decodes in) and
     stored as (c + 1) 127.5; texels with no hit are flat, (128, 128, 255).  The atlas layout is rebuilt (its texel points
     need the per-face cell records the uv do not carry) and must reproduce the mesh's uv, else ValueError.
-    ``ops.bake_normal_texture`` and include/perfb200.h state the rule.  Needs no field."""
+    ``ops.bake_normal_texture`` and include/perfb200.h state the rule.  Needs no field.  ``fill``: unused texels are filled
+    from the used ones as :func:`bake_texture`'s ``fill`` does (flat when none is used); decoding normalises the averaged
+    bytes."""
     dev = torch.device("cuda", torch.cuda.current_device())
     m = _on_gpu(mesh, dev)
     if "uv" not in m:
@@ -244,7 +263,7 @@ def bake_normal_texture(mesh: dict, source: dict, distance: float, size: Optiona
         raise ValueError(f"bake_normal_texture: the mesh's uv are not the {size}^2 texture atlas of its faces")
     src = _on_gpu(source, dev)
     normal = {"source": src, "normals": m.get("normals"), "distance": float(distance)}
-    out = _bake(None, None, None, None, m["vertices"], m["faces"], int(size), normal=normal, atlas=atlas)
+    out = _bake(None, None, None, None, m["vertices"], m["faces"], int(size), normal=normal, atlas=atlas, fill=fill)
     return dict(mesh, normal_texture=out["normal_texture"], normal_texture_hit_share=out["normal_texture_hit_share"])
 
 

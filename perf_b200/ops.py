@@ -1472,6 +1472,35 @@ def texture_views(points: torch.Tensor, face: torch.Tensor, face_normals: torch.
     return rgb, weight, view
 
 
+def texture_fill(image: torch.Tensor, used: torch.Tensor, empty=(0, 0, 0)) -> torch.Tensor:
+    """``image`` [T,T,3] uint8 (T a power of two in [256, 16384]) with its unused texels (``used`` [T,T] bool false) filled by
+    pull-push: each takes the rounded mean of the used texels of the smallest aligned 2^l x 2^l block (l >= 1) around it that
+    has any, ``empty`` (3 bytes) when no texel is used; used texels keep their bytes.  Every block of every level then
+    lies per channel within the range of its used texels, so a box-filtered mip chain never darkens towards unused texels.
+    Returns a new tensor (``perf_texture_fill``; include/perfb200.h states the rule)."""
+    image, used = _chk(image, torch.uint8, "image"), _chk(used, torch.bool, "used")
+    if image.dim() != 3 or image.shape[2] != 3 or image.shape[0] != image.shape[1] or tuple(used.shape) != tuple(image.shape[:2]):
+        raise ValueError(f"texture_fill: image {tuple(image.shape)}, used {tuple(used.shape)}: needs [T,T,3] and [T,T]")
+    T = image.shape[0]
+    if not (256 <= T <= 16384 and T & (T - 1) == 0):
+        raise ValueError(f"texture_fill: texture size {T}: needs a power of two in [256, 16384]")
+    empty = [int(e) for e in empty]
+    if len(empty) != 3 or not all(0 <= e <= 255 for e in empty):
+        raise ValueError(f"texture_fill: empty must be 3 bytes, got {empty}")
+    dev = image.device
+    if used.device != dev:
+        raise ValueError("texture_fill: image and used must be on one device")
+    # the kernels move the tiles in 16-byte pieces
+    image = image if image.data_ptr() % 16 == 0 else image.clone()
+    used = used if used.data_ptr() % 16 == 0 else used.clone()
+    out = torch.empty_like(image)
+    ws = torch.empty(int(_L().perf_texture_fill_workspace_bytes(T)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_texture_fill, _p(image), _p(used), T, (C.c_uint8 * 3)(*empty), _p(ws), ws.numel(), _p(out), _stream(),
+              launches=3 + (T > 1024))
+    return out
+
+
 def morton_xy(m: torch.Tensor):
     """(x, y) of Morton indices m (int64): x from the even bits, y from the odd bits."""
     def compact(v):

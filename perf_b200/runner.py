@@ -218,7 +218,10 @@ class CoreRunner:
         written as ``<OBJ stem>_normal.png`` with a ``norm`` line in the MTL.  With ``mesh_texture_atlas: charts`` (needs
         ``mesh_texture_size``; default ``faces``) the texture uses the chart atlas (``mesh.bake_texture``'s ``atlas``) and the
         OBJ stem gets ``_charts`` before ``_views`` (``<stem>_charts.obj``, ``<stem>_charts_views.obj``); the PLY does not
-        change.  With ``mesh_report: true`` the written mesh
+        change.  With ``mesh_texture_fill: true`` (needs ``mesh_texture_size``) the textures' unused texels are filled from
+        the used ones (``mesh.bake_texture``'s ``fill``), so mipmaps a viewer builds do not darken, and the OBJ stem gets
+        ``_fill`` last (``<stem>[_charts][_views]_fill.obj``), so an unfilled export is never overwritten; the PLY and the
+        report do not change.  With ``mesh_report: true`` the written mesh
         is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
         (path, mesh) on rank 0, else (None, None)."""
         from .mesh import write_obj, write_ply
@@ -237,6 +240,9 @@ class CoreRunner:
             raise ValueError(f"mesh_texture_atlas must be faces or charts, got {layout!r}")
         if layout != "faces" and tex is None:
             raise ValueError("mesh_texture_atlas lays out the texture: it needs mesh_texture_size")
+        fill = bool(self.conf.get("mesh_texture_fill", False))
+        if fill and tex is None:
+            raise ValueError("mesh_texture_fill fills the texture atlas's unused texels: it needs mesh_texture_size")
         mc, cut = self.conf.get("mesh_min_component", None), self.conf.get("mesh_max_cut", None)
         clean = {} if mc is None and cut is None else {"min_component": None if mc is None else float(mc),
                                                        "max_cut": None if cut is None else float(cut)}
@@ -244,6 +250,8 @@ class CoreRunner:
             clean["texture_views"] = self.sup_pool
         if layout != "faces":
             clean["atlas"] = layout
+        if fill:
+            clean["texture_fill"] = True
         if bool(self.conf.get("mesh_normal_texture", False)):
             if tex is None or target is None:
                 raise ValueError("mesh_normal_texture bakes into the decimated mesh's atlas: it needs mesh_texture_size and "
@@ -265,7 +273,8 @@ class CoreRunner:
         path = pjoin(self.exp_dir, "mesh", name)
         write_ply(path, mesh)
         if tex is not None:
-            write_obj(path[:-len(".ply")] + ("_charts" if layout == "charts" else "") + ("_views.obj" if views else ".obj"), mesh)
+            write_obj(path[:-len(".ply")] + ("_charts" if layout == "charts" else "") + ("_views" if views else "") +
+                      ("_fill.obj" if fill else ".obj"), mesh)
         if bool(self.conf.get("mesh_report", False)):
             self.mesh_report(mesh, path[:-len(".ply")], views=self.sup_pool if views else None)
         return path, mesh

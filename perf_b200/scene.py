@@ -476,18 +476,19 @@ class NeRFScene:
 
     def extract_mesh(self, resolution=512, threshold=None, colors=True, normals=True, target_faces=None, texture_size=None,
                      min_component=None, max_cut=None, texture_views=None, normal_texture=False,
-                     normal_texture_distance=None, atlas="faces") -> dict:
+                     normal_texture_distance=None, atlas="faces", texture_fill=False) -> dict:
         """Triangle mesh of the density field (:func:`perf_b200.mesh.extract_mesh` on ``self.nerf``), decimated to about
         ``target_faces`` faces when that is given, with its colour baked into a ``texture_size`` texture atlas when that is;
         ``min_component`` / ``max_cut`` (voxels) remove floaters and short handles; ``texture_views`` (registered panoramas,
         e.g. a ``SupInfoPool``) colours the texels they see from them; ``normal_texture`` bakes the full-resolution surface,
         searched within ``normal_texture_distance`` voxels (default ``mesh.NORMAL_TEXTURE_DISTANCE``), into a normal texture;
-        ``atlas`` ("faces" or "charts") selects the texture layout."""
+        ``atlas`` ("faces" or "charts") selects the texture layout; ``texture_fill`` fills the textures' unused texels from
+        the used ones (pull-push), so mipmaps a viewer builds do not darken."""
         from .mesh import DEFAULT_THRESHOLD, NORMAL_TEXTURE_DISTANCE, extract_mesh
         return extract_mesh(self.nerf, resolution, DEFAULT_THRESHOLD if threshold is None else threshold, colors, normals,
                             target_faces, texture_size, min_component=min_component, max_cut=max_cut, texture_views=texture_views,
                             normal_texture=normal_texture, normal_texture_distance=NORMAL_TEXTURE_DISTANCE
-                            if normal_texture_distance is None else normal_texture_distance, atlas=atlas)
+                            if normal_texture_distance is None else normal_texture_distance, atlas=atlas, texture_fill=texture_fill)
 
     @torch.no_grad()
     def get_pano_visibility_mask(self, sup_pool, rays: Rays):
