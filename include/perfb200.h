@@ -572,6 +572,12 @@ int perf_mesh_shade_normal_texture(const void* d_hits, const float* d_rays_d, ui
                                    const int32_t* d_faces, uint64_t F, const uint8_t* d_colors, const float* d_normals, const float* d_uv,
                                    const uint8_t* d_texture, const uint8_t* d_normal_texture, int T, float* d_rgb, float* d_distance,
                                    float* d_opacity, float* d_normal, uint8_t* d_back, void* stream);
+/* d_tangents [F,3,3]: per face and corner the unit tangent t_k of the frame above (the one the normal texture is baked and
+ * shaded with; 0 where T_f - n_k (n_k . T_f) is 0), from the low mesh (d_normals nullable) and its atlas d_uv [F,3,2].  A
+ * glTF viewer's TBN with these tangents (w = +1), the interpolated vertex normals and B = N x T reproduces the frame at the
+ * corners. */
+int perf_mesh_corner_tangents(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const float* d_normals,
+                              const float* d_uv, float* d_tangents, void* stream);
 
 /* ---- texture colour from registered panoramas (ops.texture_views drives it; csrc/texture_views.cu).  One thread per texel
  * point p of face f = d_face[i] (d_face -1: unused texel); d_face_normal [F,3] the unit geometric normals n (faces point into
@@ -622,6 +628,43 @@ int perf_texture_views(const float* d_points, const int32_t* d_face, uint64_t N,
 uint64_t perf_texture_fill_workspace_bytes(int size);     /* 0 for a size outside the rule */
 int perf_texture_fill(const uint8_t* d_image, const uint8_t* d_used, int size, const uint8_t* h_empty, void* d_workspace,
                       uint64_t workspace_bytes, uint8_t* d_out, void* stream);
+
+/* ---- PNG encoder (ops.png_encode drives it; csrc/png.cu).  d_image [H,W,3] uint8 RGB, row 0 at the top; 1 <= H and
+ * 1 <= W <= 21844 (a filtered row, 1 + 3 W bytes, fits a stored block), else PERF_EINVAL.  The file, byte for byte:
+ *   Filter: each row takes the filter type f in {0 None, 1 Sub, 2 Up, 3 Average, 4 Paeth} (bpp 3; the row above row 0 and
+ *   the bytes left of a row are 0) of the smallest sum over the row of |residual as int8|, the lower type on a tie (libpng's
+ *   heuristic).  Filtered stream: per row f, then the 3 W residuals.
+ *   Segments: consecutive whole rows, floor(65535 / (1 + 3 W)) per segment (the last may have fewer); each segment is
+ *   compressed on its own, nothing refers back across a segment start.
+ *   Tokens: per maximal run [rs, re) of equal bytes of a segment: byte rs is a literal; the remaining r = re - rs - 1 bytes
+ *   are matches at distance 1 of min(258, left) while left >= 3, then 1-2 literals.
+ *   Huffman codes (literal / length: symbols 0-285 with end-of-block 256 counted once; code lengths: symbols 0-18): the used
+ *   symbols (fewer than two: the lowest unused symbols join with count 0) sorted by (count, symbol); the two-queue Huffman
+ *   tree over them (of two smallest-weight candidates a leaf before an internal node of equal weight); leaf depths capped at
+ *   the limit (15, code lengths 7); then, while the Kraft sum sum 2^(limit - len) exceeds 2^limit, one length count at the
+ *   limit is dropped and one at the longest length l < limit that has any moves to l + 1 with a second added there (miniz's
+ *   rule); the counts are handed out from the limit down to 1 in sorted order (the rarest symbols get the longest codes).
+ *   Codes are the canonical codes of RFC 1951 3.2.2.  The distance code is two codes of length 1 (distance 1 is code 0).
+ *   Block: BFINAL 0, BTYPE 2; HLIT = max(257, last used literal / length symbol + 1), HDIST = 2, HCLEN = max(4, the
+ *   last nonzero code-length length in RFC order + 1).  The HLIT + 2 lengths as one sequence, per run of n equal values v:
+ *   v = 0: 18 with min(n, 138) while n >= 11, then 17 with n if n >= 3, the rest literal 0s; v > 0: literal v, then 16 with
+ *   min(left, 6) while left >= 3, the rest literal v.  Then the tokens, end-of-block, and an empty stored block (sync flush:
+ *   3 zero bits, padding to a byte, 00 00 ff ff).  When that is more bytes than 5 + n (a stored block of the n bytes:
+ *   00, LEN, NLEN little-endian, the bytes), the segment is that stored block instead.
+ *   Stream: 78 01, the segments, the final empty fixed-Huffman block 03 00, the Adler-32 of the filtered stream
+ *   (big-endian, combined from per-segment sums).
+ *   File: the PNG signature, IHDR (W, H, 8, 2, 0, 0, 0), one IDAT per segment (the first starts with 78 01, the last ends
+ *   with 03 00 and the Adler-32), IEND; every chunk with its CRC-32.
+ * Integer arithmetic only; the bytes do not depend on execution order.
+ * Calls, in order: perf_png_workspace_bytes(H, W) bytes of d_workspace (16-byte aligned; about H (1 + 3 W) + 65544 per
+ * segment) and perf_png_max_bytes(H, W) bytes of d_out (every segment stored); perf_png_compress (3 launches: filter,
+ * segments, finish) then perf_png_write (1 launch: the file into d_out, its size into d_file_bytes[0]).  The caller copies
+ * the size, then that many bytes of d_out. */
+uint64_t perf_png_workspace_bytes(int H, int W);           /* 0 outside the limits */
+uint64_t perf_png_max_bytes(int H, int W);                 /* 0 outside the limits */
+int perf_png_compress(const uint8_t* d_image, int H, int W, void* d_workspace, uint64_t workspace_bytes, void* stream);
+int perf_png_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
+                   uint64_t* d_file_bytes, void* stream);
 
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so

@@ -409,13 +409,11 @@ __host__ __device__ __forceinline__ void nt_cross(const float (&a)[3], const flo
     c[2] = PERF_FSUB_RN(PERF_FMUL_RN(a[0], b[1]), PERF_FMUL_RN(a[1], b[0]));
 }
 
-// MikkTSpace's frame for per-face charts (no corner is welded across faces) at barycentrics w of a face with edges e1, e2,
-// geometric normal g = e1 x e2 and corner uv[6]: the face tangent T_f from the uv differences, per corner t_k = T_f made
-// orthogonal to n_k (the vertex normal, or the unit geometric normal without vertex normals) and normalised, then the
-// unnormalised blends n = sum w_k n_k, t = sum w_k t_k and the bitangent b = n x t (sign +1: every chart has positive area).
-__host__ __device__ __forceinline__ void nt_frame(const float (&e1)[3], const float (&e2)[3], const float (&g)[3], const float* normals,
-                                                  const int32_t (&v)[3], const float* uv, const float (&w)[3], float (&t)[3],
-                                                  float (&b)[3], float (&n)[3])
+// MikkTSpace's corner frames for per-face charts (no corner is welded across faces) of a face with edges e1, e2, geometric
+// normal g = e1 x e2 and corner uv[6]: the face tangent T_f from the uv differences, per corner n_k (the vertex normal, or
+// the unit geometric normal without vertex normals) and t_k = T_f made orthogonal to n_k and normalised.
+__host__ __device__ __forceinline__ void nt_corners(const float (&e1)[3], const float (&e2)[3], const float (&g)[3], const float* normals,
+                                                    const int32_t (&v)[3], const float* uv, float (&nk)[3][3], float (&tk)[3][3])
 {
     const float du1 = PERF_FSUB_RN(uv[2], uv[0]), dv1 = PERF_FSUB_RN(uv[3], uv[1]);
     const float du2 = PERF_FSUB_RN(uv[4], uv[0]), dv2 = PERF_FSUB_RN(uv[5], uv[1]);
@@ -424,7 +422,6 @@ __host__ __device__ __forceinline__ void nt_frame(const float (&e1)[3], const fl
     for (int d = 0; d < 3; ++d) tf[d] = PERF_FDIV_RN(PERF_FSUB_RN(PERF_FMUL_RN(dv2, e1[d]), PERF_FMUL_RN(dv1, e2[d])), den);
     const float gl = PERF_FSQRT_RN(nt_dot(g, g));
     for (int d = 0; d < 3; ++d) gh[d] = gl > 0.0f ? PERF_FDIV_RN(g[d], gl) : 0.0f;
-    float nk[3][3], tk[3][3];
     for (int k = 0; k < 3; ++k) {
         float u[3];
         for (int d = 0; d < 3; ++d) nk[k][d] = normals ? normals[3 * (int64_t)v[k] + d] : gh[d];
@@ -433,6 +430,16 @@ __host__ __device__ __forceinline__ void nt_frame(const float (&e1)[3], const fl
         const float ul = PERF_FSQRT_RN(nt_dot(u, u));
         for (int d = 0; d < 3; ++d) tk[k][d] = ul > 0.0f ? PERF_FDIV_RN(u[d], ul) : 0.0f;
     }
+}
+
+// The frame at barycentrics w: the unnormalised blends n = sum w_k n_k, t = sum w_k t_k of nt_corners and the bitangent
+// b = n x t (sign +1: every chart has positive area).
+__host__ __device__ __forceinline__ void nt_frame(const float (&e1)[3], const float (&e2)[3], const float (&g)[3], const float* normals,
+                                                  const int32_t (&v)[3], const float* uv, const float (&w)[3], float (&t)[3],
+                                                  float (&b)[3], float (&n)[3])
+{
+    float nk[3][3], tk[3][3];
+    nt_corners(e1, e2, g, normals, v, uv, nk, tk);
     for (int d = 0; d < 3; ++d) {
         n[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], nk[0][d]), PERF_FMUL_RN(w[1], nk[1][d])), PERF_FMUL_RN(w[2], nk[2][d]));
         t[d] = PERF_FADD_RN(PERF_FADD_RN(PERF_FMUL_RN(w[0], tk[0][d]), PERF_FMUL_RN(w[1], tk[1][d])), PERF_FMUL_RN(w[2], tk[2][d]));
@@ -626,6 +633,20 @@ __host__ __device__ __forceinline__ void bake_texel(const BakeArgs& a, int64_t i
     a.offset[i] = off;
 }
 
+// ---------------------------------------------------------------- corner tangents (perf_mesh_corner_tangents)
+struct TangentArgs { const float* pos; const int32_t* faces; const float* normals; const float* uv; int64_t F; float* out; };
+
+// Face f: the unit corner tangents t_k of nt_corners, the ones the normal texture is baked and shaded with.
+__host__ __device__ __forceinline__ void corner_tangents(const TangentArgs& a, int64_t f)
+{
+    int32_t v[3];
+    float p[3][3], e1[3], e2[3], g[3], nk[3][3], tk[3][3];
+    load_face(a.pos, a.faces, (int32_t)f, v, p, e1, e2, g);
+    nt_corners(e1, e2, g, a.normals, v, a.uv + 6 * f, nk, tk);
+    for (int k = 0; k < 3; ++k)
+        for (int d = 0; d < 3; ++d) a.out[9 * f + 3 * k + d] = tk[k][d];
+}
+
 // ---------------------------------------------------------------- kernels
 enum { BVH_CODES, BVH_TOPOLOGY, BVH_BOXES };
 
@@ -679,6 +700,12 @@ __global__ void __launch_bounds__(128) normal_texture_bake_kernel(const BakeArgs
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < a.N) bake_texel(a, i);
+}
+
+__global__ void __launch_bounds__(128) mesh_corner_tangents_kernel(const TangentArgs a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f < a.F) corner_tangents(a, f);
 }
 
 // The product library launches the kernels; the test harness build runs the same bodies over host arrays.
@@ -892,6 +919,26 @@ int perf_normal_texture_bake(const int32_t* d_nodes, const float* d_tris, const 
     for (int64_t i = 0; i < a.N; ++i) bake_texel(a, i);
 #else
     normal_texture_bake_kernel<<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a);
+    PERF_LAUNCH_CHECK();
+#endif
+    return PERF_OK;
+}
+
+int perf_mesh_corner_tangents(const float* d_vertices, uint64_t V, const int32_t* d_faces, uint64_t F, const float* d_normals,
+                              const float* d_uv, float* d_tangents, void* stream)
+{
+    if (F == 0) return PERF_OK;
+    PERF_CHECK_ARG(V < (1ull << 31) && F < (1ull << 30), "mesh of %llu vertices / %llu faces: needs V < 2^31 and F < 2^30",
+                   (unsigned long long)V, (unsigned long long)F);
+    PERF_CHECK_ARG(d_vertices && d_faces && d_uv && d_tangents, "NULL pointer");
+    TangentArgs a;
+    memset(&a, 0, sizeof(a));
+    a.pos = d_vertices; a.faces = d_faces; a.normals = d_normals; a.uv = d_uv; a.F = (int64_t)F; a.out = d_tangents;
+#ifdef PERF_HOST_HARNESS
+    (void)stream;
+    for (int64_t f = 0; f < a.F; ++f) corner_tangents(a, f);
+#else
+    mesh_corner_tangents_kernel<<<(unsigned)((F + 127) / 128), 128, 0, (cudaStream_t)stream>>>(a);
     PERF_LAUNCH_CHECK();
 #endif
     return PERF_OK;

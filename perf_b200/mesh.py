@@ -424,6 +424,230 @@ def read_obj(path: str) -> dict:
     return out
 
 
+GLB_MAX_BYTES = 2 ** 32 - 1        # the GLB header's length field
+_GLB_JSON_MAX = 1 << 14             # the JSON chunk write_glb writes is under 2 KB
+_SRGB8_LINEAR = np.asarray([c / 12.92 if c <= 0.04045 else ((c + 0.055) / 1.055) ** 2.4 for c in np.arange(256) / 255.0], np.float32)
+_SRGB8_MID = (_SRGB8_LINEAR[:-1].astype(np.float64) + _SRGB8_LINEAR[1:]) / 2
+
+
+def _pad4(n: int) -> int:
+    return (n + 3) & ~3
+
+
+def glb_bytes(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=()) -> int:
+    """An upper bound of the size of the GLB :func:`write_glb` writes, from counts alone: ``vertices`` glTF vertices (after
+    the per-face atlas's split), ``indices`` uint32 indices (0 for a non-indexed primitive), the attributes present and the
+    PNG ``images`` byte counts."""
+    per_vertex = 12 + 12 * bool(normals) + 12 * bool(colors) + 8 * bool(uv) + 16 * bool(tangents)
+    bin_ = per_vertex * int(vertices) + 4 * int(indices) + sum(_pad4(int(n)) for n in images)
+    return 12 + 8 + _GLB_JSON_MAX + 8 + bin_
+
+
+def check_glb_size(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=()) -> None:
+    """ValueError when :func:`glb_bytes` exceeds 2^32 - 1, the largest GLB the format's 32-bit length field can state."""
+    n = glb_bytes(vertices, indices, normals, colors, uv, tangents, images)
+    if n > GLB_MAX_BYTES:
+        raise ValueError(f"write_glb: {vertices} vertices and {indices} indices make a GLB of up to {n} bytes, over the format's "
+                         f"limit of 2^32 - 1")
+
+
+def write_glb(path: str, mesh: dict) -> None:
+    """One binary glTF 2.0 file of an :func:`extract_mesh` / :func:`bake_texture` / :func:`bake_normal_texture` result: one
+    mesh of one triangle primitive under one node whose rotation (-sqrt(1/2), 0, 0, sqrt(1/2)) turns PeRF's +Z-up world into
+    glTF's +Y-up (the vertex data stay in world coordinates).  fp32 ``POSITION`` (with min / max) and ``NORMAL`` when the mesh
+    has normals; no quantisation, so every value reads back exactly.
+    Without a texture: the vertices as they are, uint32 indices, ``COLOR_0`` the colours as linear fp32 (sRGB bytes decoded,
+    as the spec defines ``COLOR_0``), an unlit material (``KHR_materials_unlit``: the colour already holds the scene's light).
+    Per-face atlas: one vertex per face corner in face order, no indices, ``TEXCOORD_0`` = (u, 1 - v), the albedo as an
+    embedded PNG (``ops.png_encode``) in ``baseColorTexture``, no ``COLOR_0`` (glTF would multiply it into the texture).
+    Chart atlas (``"uv_faces"``): one vertex per uv vertex at its mesh vertex, ``uv_faces`` as the indices.  With
+    ``"normal_texture"`` (per-face atlas): ``normalTexture`` and ``TANGENT`` = (t_k, +1) per corner (``ops.corner_tangents``:
+    the tangents the texture was baked in), and the material is lit PBR, metallic 0, roughness 1.  Triangles face free space
+    counter-clockwise, so the material is single-sided.  ValueError before anything is written when the file would exceed
+    2^32 - 1 bytes (:func:`check_glb_size`)."""
+    import json
+    import struct
+    from . import ops
+    tex = mesh.get("texture")
+    ntex = mesh.get("normal_texture")
+    charts = mesh.get("uv_faces") is not None
+    if ntex is not None and (tex is None or charts):
+        raise ValueError("write_glb: a normal texture is written with the per-face atlas's albedo texture")
+    faces_t = mesh["faces"]
+    F = int(faces_t.shape[0]) if faces_t.ndim == 2 else int(faces_t.shape[0]) // 3
+    has_n = mesh.get("normals") is not None
+    if tex is None:
+        V, n_idx = int(mesh["vertices"].shape[0]), 3 * F
+    elif charts:
+        V, n_idx = int(mesh["uv_vertices"].shape[0]), 3 * F
+    else:
+        V, n_idx = 3 * F, 0
+    colors = tex is None and mesh.get("colors") is not None
+    check_glb_size(V, n_idx, has_n, colors, tex is not None, ntex is not None)
+    images = []
+    if tex is not None:
+        images.append(ops.png_encode(_cuda_u8(tex)))
+        if ntex is not None:
+            images.append(ops.png_encode(_cuda_u8(ntex)))
+        check_glb_size(V, n_idx, has_n, colors, True, ntex is not None, [len(b) for b in images])
+
+    verts = np.ascontiguousarray(_np(mesh["vertices"]), np.float32).reshape(-1, 3)
+    faces = np.ascontiguousarray(_np(faces_t), np.int64).reshape(-1, 3)
+    nrm = np.ascontiguousarray(_np(mesh["normals"]), np.float32).reshape(-1, 3) if has_n else None
+    attrs, indices = {}, None
+    if tex is None:
+        attrs["POSITION"] = verts
+        if has_n:
+            attrs["NORMAL"] = nrm
+        if colors:
+            attrs["COLOR_0"] = _SRGB8_LINEAR[np.asarray(_np(mesh["colors"]), np.uint8).reshape(-1, 3)]
+        indices = faces.astype(np.uint32)
+    elif charts:
+        uvf = np.ascontiguousarray(_np(mesh["uv_faces"]), np.int64).reshape(-1, 3)
+        vmap = np.zeros(V, np.int64)
+        vmap[uvf.reshape(-1)] = faces.reshape(-1)
+        uvv = np.ascontiguousarray(_np(mesh["uv_vertices"]), np.float32).reshape(-1, 2)
+        attrs["POSITION"] = verts[vmap]
+        if has_n:
+            attrs["NORMAL"] = nrm[vmap]
+        attrs["TEXCOORD_0"] = np.stack([uvv[:, 0], np.float32(1) - uvv[:, 1]], 1)
+        indices = uvf.astype(np.uint32)
+    else:
+        corner = faces.reshape(-1)
+        uv = np.ascontiguousarray(_np(mesh["uv"]), np.float32).reshape(-1, 2)
+        attrs["POSITION"] = verts[corner]
+        if has_n:
+            attrs["NORMAL"] = nrm[corner]
+        attrs["TEXCOORD_0"] = np.stack([uv[:, 0], np.float32(1) - uv[:, 1]], 1)
+        if ntex is not None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+            m = _on_gpu(mesh, dev)
+            t = ops.corner_tangents(m["vertices"], m["faces"], m.get("normals"), m["uv"]).reshape(-1, 3).cpu().numpy()
+            attrs["TANGENT"] = np.concatenate([t, np.ones((t.shape[0], 1), np.float32)], 1)
+
+    blobs, views, accessors = [], [], []
+
+    def view(data: bytes, target=None) -> int:
+        off = sum(len(b) for b in blobs)
+        blobs.append(data + b"\0" * (_pad4(len(data)) - len(data)))
+        v = {"buffer": 0, "byteOffset": off, "byteLength": len(data)}
+        if target:
+            v["target"] = target
+        views.append(v)
+        return len(views) - 1
+
+    types = {1: "SCALAR", 2: "VEC2", 3: "VEC3", 4: "VEC4"}
+    prim = {"attributes": {}, "mode": 4, "material": 0}
+    for name, a in attrs.items():
+        a = np.ascontiguousarray(a, np.float32)
+        acc = {"bufferView": view(a.tobytes(), 34962), "componentType": 5126, "count": int(a.shape[0]), "type": types[a.shape[1]]}
+        if name == "POSITION":
+            acc["min"] = [float(x) for x in a.min(0)] if len(a) else [0.0] * 3
+            acc["max"] = [float(x) for x in a.max(0)] if len(a) else [0.0] * 3
+        accessors.append(acc)
+        prim["attributes"][name] = len(accessors) - 1
+    if indices is not None:
+        accessors.append({"bufferView": view(indices.reshape(-1).tobytes(), 34963), "componentType": 5125,
+                          "count": int(indices.size), "type": "SCALAR"})
+        prim["indices"] = len(accessors) - 1
+    material = {"pbrMetallicRoughness": {"baseColorFactor": [1.0, 1.0, 1.0, 1.0], "metallicFactor": 0.0, "roughnessFactor": 1.0},
+                "doubleSided": False}
+    doc = {"asset": {"version": "2.0", "generator": "perf_b200.mesh.write_glb"}, "scene": 0, "scenes": [{"nodes": [0]}],
+           "nodes": [{"mesh": 0, "rotation": [-float(np.sqrt(0.5)), 0.0, 0.0, float(np.sqrt(0.5))]}],
+           "meshes": [{"primitives": [prim]}], "materials": [material]}
+    if images:
+        doc["images"] = [{"bufferView": view(b), "mimeType": "image/png"} for b in images]
+        doc["samplers"] = [{"magFilter": 9729, "minFilter": 9987, "wrapS": 33071, "wrapT": 33071}]
+        doc["textures"] = [{"sampler": 0, "source": i} for i in range(len(images))]
+        material["pbrMetallicRoughness"]["baseColorTexture"] = {"index": 0}
+        if ntex is not None:
+            material["normalTexture"] = {"index": 1}
+    if ntex is None:
+        material["extensions"] = {"KHR_materials_unlit": {}}
+        doc["extensionsUsed"] = ["KHR_materials_unlit"]
+    doc["accessors"], doc["bufferViews"] = accessors, views
+    bin_len = sum(len(b) for b in blobs)
+    doc["buffers"] = [{"byteLength": bin_len}]
+    js = json.dumps(doc, separators=(",", ":")).encode("ascii")
+    js += b" " * (_pad4(len(js)) - len(js))
+    assert len(js) <= _GLB_JSON_MAX
+    total = 12 + 8 + len(js) + 8 + bin_len
+    with open(path, "wb") as f:
+        f.write(struct.pack("<III", 0x46546C67, 2, total))
+        f.write(struct.pack("<II", len(js), 0x4E4F534A))
+        f.write(js)
+        f.write(struct.pack("<II", bin_len, 0x004E4942))
+        for b in blobs:
+            f.write(b)
+
+
+def _cuda_u8(a) -> torch.Tensor:
+    t = a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+    return t.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.uint8).contiguous()
+
+
+def read_glb(path: str) -> dict:
+    """Reads what :func:`write_glb` writes (numpy arrays), with :func:`read_obj`'s keys: vertices, faces (``arange`` for the
+    per-face atlas's non-indexed primitive), normals, colors (sRGB bytes again), uv [F,3,2] (v up again; with ``uv_vertices``
+    / ``uv_faces`` for an indexed textured primitive, the chart atlas), texture and normal_texture (RGB), and ``tangents``
+    [V,4].  Also ``"gltf"``, the JSON document."""
+    import json
+    import struct
+    import cv2
+    with open(path, "rb") as f:
+        data = f.read()
+    magic, version, total = struct.unpack_from("<III", data, 0)
+    if magic != 0x46546C67 or version != 2 or total != len(data):
+        raise ValueError(f"read_glb: {path} is not a GLB 2.0 file")
+    jl, jt = struct.unpack_from("<II", data, 12)
+    doc = json.loads(data[20:20 + jl])
+    bl, bt = struct.unpack_from("<II", data, 20 + jl)
+    if jt != 0x4E4F534A or bt != 0x004E4942:
+        raise ValueError(f"read_glb: {path}: unexpected chunk types")
+    binary = data[28 + jl:28 + jl + bl]
+
+    def view(i):
+        v = doc["bufferViews"][i]
+        return binary[v.get("byteOffset", 0):v.get("byteOffset", 0) + v["byteLength"]]
+
+    def accessor(i):
+        a = doc["accessors"][i]
+        dt = {5126: np.float32, 5125: np.uint32}[a["componentType"]]
+        k = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4}[a["type"]]
+        return np.frombuffer(view(a["bufferView"]), dt, count=a["count"] * k).reshape(a["count"], k).copy()
+
+    prim = doc["meshes"][0]["primitives"][0]
+    at = prim["attributes"]
+    verts = accessor(at["POSITION"])
+    faces = (accessor(prim["indices"]).reshape(-1, 3).astype(np.int32) if "indices" in prim
+             else np.arange(verts.shape[0], dtype=np.int32).reshape(-1, 3))
+    out = {"vertices": verts, "faces": faces, "gltf": doc}
+    if "NORMAL" in at:
+        out["normals"] = accessor(at["NORMAL"])
+    if "COLOR_0" in at:
+        out["colors"] = np.searchsorted(_SRGB8_MID, accessor(at["COLOR_0"])[:, :3].astype(np.float64)).astype(np.uint8)
+    if "TANGENT" in at:
+        out["tangents"] = accessor(at["TANGENT"])
+    if "TEXCOORD_0" in at:
+        tc = accessor(at["TEXCOORD_0"])
+        uvv = np.stack([tc[:, 0], np.float32(1) - tc[:, 1]], 1)
+        out["uv"] = uvv[faces]
+        if "indices" in prim:
+            out["uv_vertices"], out["uv_faces"] = uvv, faces.copy()
+    mat = doc["materials"][prim["material"]] if "material" in prim else {}
+
+    def image(tex):
+        img = doc["images"][doc["textures"][tex["index"]]["source"]]
+        dec = cv2.imdecode(np.frombuffer(view(img["bufferView"]), np.uint8), cv2.IMREAD_UNCHANGED)
+        return np.ascontiguousarray(dec[:, :, ::-1])
+
+    if "baseColorTexture" in mat.get("pbrMetallicRoughness", {}):
+        out["texture"] = image(mat["pbrMetallicRoughness"]["baseColorTexture"])
+    if "normalTexture" in mat:
+        out["normal_texture"] = image(mat["normalTexture"])
+    return out
+
+
 def _np(a) -> np.ndarray:
     return a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
 

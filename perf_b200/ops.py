@@ -1501,6 +1501,48 @@ def texture_fill(image: torch.Tensor, used: torch.Tensor, empty=(0, 0, 0)) -> to
     return out
 
 
+PNG_MAX_WIDTH = 21844       # a filtered row, 1 + 3 W bytes, fits one stored deflate block
+
+
+def png_encode(image: torch.Tensor) -> bytes:
+    """A complete PNG (8-bit RGB, no interlace) of ``image`` [H,W,3] uint8, row 0 at the top, 1 <= W <= 21844, compressed on
+    the GPU (``perf_png_compress`` / ``perf_png_write``; include/perfb200.h states every byte): per row the libpng filter
+    heuristic, independent deflate segments of whole rows whose matches are runs (distance 1) parsed in closed form, one
+    dynamic-Huffman block per segment (stored when that is shorter), per-chunk CRC-32 and the combined Adler-32.  The host
+    copies the file size, then the file."""
+    image = _chk(image, torch.uint8, "image")
+    if image.dim() != 3 or image.shape[2] != 3 or image.shape[0] < 1 or not 1 <= image.shape[1] <= PNG_MAX_WIDTH:
+        raise ValueError(f"png_encode: image {tuple(image.shape)}: needs [H,W,3] with H >= 1 and 1 <= W <= {PNG_MAX_WIDTH}")
+    H, W, dev = image.shape[0], image.shape[1], image.device
+    ws = torch.empty(int(_L().perf_png_workspace_bytes(H, W)), dtype=torch.uint8, device=dev)
+    out = torch.empty(int(_L().perf_png_max_bytes(H, W)), dtype=torch.uint8, device=dev)
+    size = torch.empty(1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_png_compress, _p(image), H, W, _p(ws), ws.numel(), _stream(), launches=3)
+        _call(_L().perf_png_write, _p(ws), ws.numel(), H, W, _p(out), out.numel(), _p(size), _stream())
+        n = int(size.item())
+        return out[:n].cpu().numpy().tobytes()
+
+
+def corner_tangents(vertices: torch.Tensor, faces: torch.Tensor, normals: Optional[torch.Tensor], uv: torch.Tensor) -> torch.Tensor:
+    """[F,3,3] fp32: per face corner the unit tangent of the frame the normal texture is baked and shaded with
+    (``perf_mesh_corner_tangents``: MikkTSpace's t_k for per-face charts; the vertex ``normals``, else the geometric normal,
+    and the per-face atlas ``uv`` [F,3,2])."""
+    vertices, faces = _chk(vertices, torch.float32, "vertices"), _chk(faces, torch.int32, "faces").reshape(-1, 3)
+    uv = _chk(uv, torch.float32, "uv").reshape(-1, 3, 2)
+    if normals is not None:
+        normals = _chk(normals, torch.float32, "normals")
+        if tuple(normals.shape) != tuple(vertices.shape):
+            raise ValueError(f"corner_tangents: normals {tuple(normals.shape)} for vertices {tuple(vertices.shape)}")
+    F = faces.shape[0]
+    if uv.shape[0] != F:
+        raise ValueError(f"corner_tangents: uv for {uv.shape[0]} faces, the mesh has {F}")
+    out = torch.empty(F, 3, 3, dtype=torch.float32, device=vertices.device)
+    with torch.cuda.device(vertices.device):
+        _call(_L().perf_mesh_corner_tangents, _p(vertices), vertices.shape[0], _p(faces), F, _p(normals), _p(uv), _p(out), _stream())
+    return out
+
+
 def morton_xy(m: torch.Tensor):
     """(x, y) of Morton indices m (int64): x from the even bits, y from the odd bits."""
     def compact(v):

@@ -221,10 +221,12 @@ class CoreRunner:
         change.  With ``mesh_texture_fill: true`` (needs ``mesh_texture_size``) the textures' unused texels are filled from
         the used ones (``mesh.bake_texture``'s ``fill``), so mipmaps a viewer builds do not darken, and the OBJ stem gets
         ``_fill`` last (``<stem>[_charts][_views]_fill.obj``), so an unfilled export is never overwritten; the PLY and the
-        report do not change.  With ``mesh_report: true`` the written mesh
+        report do not change.  With ``mesh_glb: true`` the mesh is also written as one binary glTF file (``mesh.write_glb``:
+        textures PNG-encoded on the GPU, normal texture with tangents), ``<OBJ stem>.glb`` when it has a texture, else
+        ``<PLY stem>.glb``; the other files do not change.  With ``mesh_report: true`` the written mesh
         is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
         (path, mesh) on rank 0, else (None, None)."""
-        from .mesh import write_obj, write_ply
+        from .mesh import write_glb, write_obj, write_ply
         if not self.is_main:
             return None, None
         res = int(resolution if resolution is not None else self.conf.get("mesh_resolution", 512))
@@ -272,9 +274,12 @@ class CoreRunner:
             name = name[:-len(".ply")] + "_clean.ply"
         path = pjoin(self.exp_dir, "mesh", name)
         write_ply(path, mesh)
+        stem = path[:-len(".ply")]
         if tex is not None:
-            write_obj(path[:-len(".ply")] + ("_charts" if layout == "charts" else "") + ("_views" if views else "") +
-                      ("_fill.obj" if fill else ".obj"), mesh)
+            stem += ("_charts" if layout == "charts" else "") + ("_views" if views else "") + ("_fill" if fill else "")
+            write_obj(stem + ".obj", mesh)
+        if bool(self.conf.get("mesh_glb", False)):
+            write_glb(stem + ".glb", mesh)
         if bool(self.conf.get("mesh_report", False)):
             self.mesh_report(mesh, path[:-len(".ply")], views=self.sup_pool if views else None)
         return path, mesh
