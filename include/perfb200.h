@@ -666,6 +666,43 @@ int perf_png_compress(const uint8_t* d_image, int H, int W, void* d_workspace, u
 int perf_png_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
                    uint64_t* d_file_bytes, void* stream);
 
+/* ---- baseline JPEG encoder (ops.jpeg_encode drives it; csrc/jpeg.cu).  d_image [H,W,3] uint8 RGB, row 0 at the top;
+ * 1 <= H, W <= 65535 and 1 <= quality <= 100, else PERF_EINVAL.  The file is libjpeg's (IJG / libjpeg-turbo, default ISLOW
+ * path) for quality q, 4:4:4 sampling and a restart interval of ceil(W / 8) MCUs, byte for byte:
+ *   Blocks: MX = ceil(W / 8) by MY = ceil(H / 8) MCUs, each one 8 x 8 block of Y, Cb and Cr; samples past the right or bottom
+ *   edge repeat the last column or row.
+ *   Colour: Y = (19595 R + 38470 G + 7471 B + 32768) >> 16, Cb = (-11059 R - 21709 G + 32768 B + 8421375) >> 16,
+ *   Cr = (32768 R - 27439 G - 5329 B + 8421375) >> 16; the DCT input is the sample - 128.
+ *   DCT: libjpeg's jpeg_fdct_islow (LL&M; CONST_BITS 13, PASS1_BITS 2; rows, then columns; DESCALE(x, n) = (x + 2^(n-1)) >> n,
+ *   arithmetic), 32-bit integers; its outputs are 8 x the orthonormal DCT.
+ *   Quantisers: with s = 5000 / q for q < 50 and 200 - 2 q otherwise, Q = clamp((K * s + 50) / 100, 1, 255) per entry K of
+ *   the ITU-T T.81 Annex K.1 (luma) / K.2 (chroma) table.  Coefficient v -> sign(v) ((|v| + 4 Q) / (8 Q)), integer division
+ *   (libjpeg-turbo's reciprocal form gives the same value for every |v| these DCTs produce).
+ *   Entropy: the Annex K.3 / K.5 Huffman tables (DC 0 / AC 0 for Y, DC 1 / AC 1 for Cb and Cr); per block the DC difference
+ *   to the same component of the MCU to the left (0 at the start of every MCU row), then the AC run-lengths in zigzag order
+ *   with ZRL per 16 zeros before a nonzero coefficient and EOB when the block ends in zeros; magnitude bits of v < 0 are
+ *   those of v - 1.  Each MCU row is one restart interval: its bits MSB first, padded with 1 bits to a byte, every FF
+ *   followed by 00, then RST(r mod 8) after row r unless it is the last.
+ *   File: SOI; APP0 JFIF 1.01, units 0, density 1:1, no thumbnail; DQT 0 (luma) and DQT 1 (chroma), 8-bit, zigzag order; SOF0
+ *   (8-bit, H, W, components 1, 2, 3 at 1x1 with tables 0, 1, 1); DHT DC 0, AC 0, DC 1, AC 1; DRI MX; SOS (components 1, 2, 3
+ *   with tables 0/0, 1/1, 1/1; 0, 63, 0); the rows; EOI.  629 bytes precede the entropy-coded data.
+ * Integer arithmetic only; the only atomics are integer ORs, so the bytes do not depend on execution order.
+ * Calls, in order: perf_jpeg_workspace_bytes(H, W) bytes of d_workspace (16-byte aligned; 16 bytes per MCU plus, per MCU row,
+ * room for the row's unstuffed bits at the worst case of 4978 bits per MCU: about 10 bytes per pixel); perf_jpeg_compress (5
+ * launches: bits, interval, emit, count, finish); then either perf_jpeg_file_bytes (the file's exact size into
+ * d_file_bytes[0], a device-to-device copy) and, once the caller has read it, an output buffer of that size, or an output
+ * buffer of perf_jpeg_max_bytes(H, W) bytes (every row at the worst case, every byte stuffed: about 19.5 bytes per pixel)
+ * without the read; then perf_jpeg_write (1 launch): when the file fits the out_bytes of d_out, the file into d_out and its
+ * size into d_file_bytes[0]; when it does not, nothing is written and d_file_bytes[0] = 0.  out_bytes below the smallest
+ * file (631 bytes) is PERF_EINVAL.  The caller copies the size, then that many bytes of d_out. */
+uint64_t perf_jpeg_workspace_bytes(int H, int W);          /* 0 outside the limits */
+uint64_t perf_jpeg_max_bytes(int H, int W);                /* 0 outside the limits */
+int perf_jpeg_compress(const uint8_t* d_image, int H, int W, int quality, void* d_workspace, uint64_t workspace_bytes,
+                       void* stream);
+int perf_jpeg_file_bytes(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint64_t* d_file_bytes, void* stream);
+int perf_jpeg_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
+                    uint64_t* d_file_bytes, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

@@ -129,6 +129,11 @@ SIGNATURES = {
     "perf_png_max_bytes": (u64, [i32, i32]),
     "perf_png_compress": (i32, [vp, i32, i32, vp, u64, vp]),
     "perf_png_write": (i32, [vp, u64, i32, i32, vp, u64, vp, vp]),
+    "perf_jpeg_workspace_bytes": (u64, [i32, i32]),
+    "perf_jpeg_max_bytes": (u64, [i32, i32]),
+    "perf_jpeg_compress": (i32, [vp, i32, i32, i32, vp, u64, vp]),
+    "perf_jpeg_write": (i32, [vp, u64, i32, i32, vp, u64, vp, vp]),
+    "perf_jpeg_file_bytes": (i32, [vp, u64, i32, i32, vp, vp]),
     "perf_mesh_corner_tangents": (i32, [vp, u64, vp, u64, vp, vp, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -425,6 +425,9 @@ def read_obj(path: str) -> dict:
 
 
 GLB_MAX_BYTES = 2 ** 32 - 1        # the GLB header's length field
+# JPEG quality of write_glb(compact=True)'s textures: chosen from tools/bench_glb_compact.py's sweep (DESIGN §6)
+GLB_JPEG_QUALITY = 90
+_GLB_ROTATION = [-float(np.sqrt(0.5)), 0.0, 0.0, float(np.sqrt(0.5))]     # +Z up -> +Y up: (x, y, z) -> (x, z, -y)
 _GLB_JSON_MAX = 1 << 14             # the JSON chunk write_glb writes is under 2 KB
 _SRGB8_LINEAR = np.asarray([c / 12.92 if c <= 0.04045 else ((c + 0.055) / 1.055) ** 2.4 for c in np.arange(256) / 255.0], np.float32)
 _SRGB8_MID = (_SRGB8_LINEAR[:-1].astype(np.float64) + _SRGB8_LINEAR[1:]) / 2
@@ -434,24 +437,29 @@ def _pad4(n: int) -> int:
     return (n + 3) & ~3
 
 
-def glb_bytes(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=()) -> int:
+def glb_bytes(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=(), compact=False) -> int:
     """An upper bound of the size of the GLB :func:`write_glb` writes, from counts alone: ``vertices`` glTF vertices (after
-    the per-face atlas's split), ``indices`` uint32 indices (0 for a non-indexed primitive), the attributes present and the
-    PNG ``images`` byte counts."""
-    per_vertex = 12 + 12 * bool(normals) + 12 * bool(colors) + 8 * bool(uv) + 16 * bool(tangents)
+    the per-face atlas's split), ``indices`` uint32 indices (0 for a non-indexed primitive), the attributes present, the
+    ``images`` byte counts and the ``compact`` layout (quantised attributes: 8, 4, 8, 8 and 4 bytes per vertex for position,
+    normal, colour, uv and tangent, against 12, 12, 12, 8 and 16)."""
+    if compact:
+        per_vertex = 8 + 4 * bool(normals) + 8 * bool(colors) + 8 * bool(uv) + 4 * bool(tangents)
+    else:
+        per_vertex = 12 + 12 * bool(normals) + 12 * bool(colors) + 8 * bool(uv) + 16 * bool(tangents)
     bin_ = per_vertex * int(vertices) + 4 * int(indices) + sum(_pad4(int(n)) for n in images)
     return 12 + 8 + _GLB_JSON_MAX + 8 + bin_
 
 
-def check_glb_size(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=()) -> None:
+def check_glb_size(vertices: int, indices: int, normals: bool, colors: bool, uv: bool, tangents: bool, images=(),
+                   compact=False) -> None:
     """ValueError when :func:`glb_bytes` exceeds 2^32 - 1, the largest GLB the format's 32-bit length field can state."""
-    n = glb_bytes(vertices, indices, normals, colors, uv, tangents, images)
+    n = glb_bytes(vertices, indices, normals, colors, uv, tangents, images, compact)
     if n > GLB_MAX_BYTES:
         raise ValueError(f"write_glb: {vertices} vertices and {indices} indices make a GLB of up to {n} bytes, over the format's "
                          f"limit of 2^32 - 1")
 
 
-def write_glb(path: str, mesh: dict) -> None:
+def write_glb(path: str, mesh: dict, compact: bool = False) -> None:
     """One binary glTF 2.0 file of an :func:`extract_mesh` / :func:`bake_texture` / :func:`bake_normal_texture` result: one
     mesh of one triangle primitive under one node whose rotation (-sqrt(1/2), 0, 0, sqrt(1/2)) turns PeRF's +Z-up world into
     glTF's +Y-up (the vertex data stay in world coordinates).  fp32 ``POSITION`` (with min / max) and ``NORMAL`` when the mesh
@@ -464,7 +472,14 @@ def write_glb(path: str, mesh: dict) -> None:
     ``"normal_texture"`` (per-face atlas): ``normalTexture`` and ``TANGENT`` = (t_k, +1) per corner (``ops.corner_tangents``:
     the tangents the texture was baked in), and the material is lit PBR, metallic 0, roughness 1.  Triangles face free space
     counter-clockwise, so the material is single-sided.  ValueError before anything is written when the file would exceed
-    2^32 - 1 bytes (:func:`check_glb_size`)."""
+    2^32 - 1 bytes (:func:`check_glb_size`).
+    ``compact=True``: the textures as ``image/jpeg`` (``ops.jpeg_encode`` at :data:`GLB_JPEG_QUALITY`) and the attributes
+    quantised with ``KHR_mesh_quantization`` (required): ``POSITION`` normalised uint16 over the cube at the low corner of
+    the written positions' bounding box with the box's largest extent as its side (byte stride 8), undone by the node's
+    uniform ``scale`` (that extent, so viewers keep the normals' and tangents' directions) and ``translation`` (the low
+    corner, rotated) beside the rotation; ``NORMAL`` normalised int8 (stride 4); ``TANGENT`` normalised int8 x 4; ``COLOR_0`` normalised
+    uint16 linear (stride 8), which keeps every sRGB byte apart; ``TEXCOORD_0`` stays fp32.  Per vertex: 24 bytes for the
+    per-face atlas with a normal texture (48 exact), 20 for the chart atlas (32) and for an untextured mesh (36)."""
     import json
     import struct
     from . import ops
@@ -483,13 +498,14 @@ def write_glb(path: str, mesh: dict) -> None:
     else:
         V, n_idx = 3 * F, 0
     colors = tex is None and mesh.get("colors") is not None
-    check_glb_size(V, n_idx, has_n, colors, tex is not None, ntex is not None)
+    check_glb_size(V, n_idx, has_n, colors, tex is not None, ntex is not None, compact=compact)
     images = []
     if tex is not None:
-        images.append(ops.png_encode(_cuda_u8(tex)))
+        encode = (lambda t: ops.jpeg_encode(t, GLB_JPEG_QUALITY)) if compact else ops.png_encode
+        images.append(encode(_cuda_u8(tex)))
         if ntex is not None:
-            images.append(ops.png_encode(_cuda_u8(ntex)))
-        check_glb_size(V, n_idx, has_n, colors, True, ntex is not None, [len(b) for b in images])
+            images.append(encode(_cuda_u8(ntex)))
+        check_glb_size(V, n_idx, has_n, colors, True, ntex is not None, [len(b) for b in images], compact)
 
     verts = np.ascontiguousarray(_np(mesh["vertices"]), np.float32).reshape(-1, 3)
     faces = np.ascontiguousarray(_np(faces_t), np.int64).reshape(-1, 3)
@@ -527,10 +543,12 @@ def write_glb(path: str, mesh: dict) -> None:
 
     blobs, views, accessors = [], [], []
 
-    def view(data: bytes, target=None) -> int:
+    def view(data: bytes, target=None, stride=None) -> int:
         off = sum(len(b) for b in blobs)
         blobs.append(data + b"\0" * (_pad4(len(data)) - len(data)))
         v = {"buffer": 0, "byteOffset": off, "byteLength": len(data)}
+        if stride:
+            v["byteStride"] = stride
         if target:
             v["target"] = target
         views.append(v)
@@ -538,12 +556,24 @@ def write_glb(path: str, mesh: dict) -> None:
 
     types = {1: "SCALAR", 2: "VEC2", 3: "VEC3", 4: "VEC4"}
     prim = {"attributes": {}, "mode": 4, "material": 0}
+    node = {"mesh": 0, "rotation": _GLB_ROTATION}
+    if compact:
+        attrs, node_ts = _quantise_attributes(attrs)
+        node.update(node_ts)
     for name, a in attrs.items():
-        a = np.ascontiguousarray(a, np.float32)
-        acc = {"bufferView": view(a.tobytes(), 34962), "componentType": 5126, "count": int(a.shape[0]), "type": types[a.shape[1]]}
+        if not compact or a.dtype == np.float32:
+            a = np.ascontiguousarray(a, np.float32)
+            acc = {"bufferView": view(a.tobytes(), 34962), "componentType": 5126}
+        else:
+            k = {"POSITION": 3, "NORMAL": 3, "COLOR_0": 3, "TANGENT": 4}[name]
+            acc = {"bufferView": view(a.tobytes(), 34962, a.shape[1] * a.itemsize), "componentType": _GLB_COMPONENT[a.dtype.type],
+                   "normalized": True}
+            a = a[:, :k]
+        acc.update({"count": int(a.shape[0]), "type": types[a.shape[1]]})
         if name == "POSITION":
-            acc["min"] = [float(x) for x in a.min(0)] if len(a) else [0.0] * 3
-            acc["max"] = [float(x) for x in a.max(0)] if len(a) else [0.0] * 3
+            cast = float if a.dtype == np.float32 else int
+            acc["min"] = [cast(x) for x in a.min(0)] if len(a) else [cast(0)] * 3
+            acc["max"] = [cast(x) for x in a.max(0)] if len(a) else [cast(0)] * 3
         accessors.append(acc)
         prim["attributes"][name] = len(accessors) - 1
     if indices is not None:
@@ -553,10 +583,10 @@ def write_glb(path: str, mesh: dict) -> None:
     material = {"pbrMetallicRoughness": {"baseColorFactor": [1.0, 1.0, 1.0, 1.0], "metallicFactor": 0.0, "roughnessFactor": 1.0},
                 "doubleSided": False}
     doc = {"asset": {"version": "2.0", "generator": "perf_b200.mesh.write_glb"}, "scene": 0, "scenes": [{"nodes": [0]}],
-           "nodes": [{"mesh": 0, "rotation": [-float(np.sqrt(0.5)), 0.0, 0.0, float(np.sqrt(0.5))]}],
+           "nodes": [node],
            "meshes": [{"primitives": [prim]}], "materials": [material]}
     if images:
-        doc["images"] = [{"bufferView": view(b), "mimeType": "image/png"} for b in images]
+        doc["images"] = [{"bufferView": view(b), "mimeType": "image/jpeg" if compact else "image/png"} for b in images]
         doc["samplers"] = [{"magFilter": 9729, "minFilter": 9987, "wrapS": 33071, "wrapT": 33071}]
         doc["textures"] = [{"sampler": 0, "source": i} for i in range(len(images))]
         material["pbrMetallicRoughness"]["baseColorTexture"] = {"index": 0}
@@ -565,6 +595,9 @@ def write_glb(path: str, mesh: dict) -> None:
     if ntex is None:
         material["extensions"] = {"KHR_materials_unlit": {}}
         doc["extensionsUsed"] = ["KHR_materials_unlit"]
+    if compact:
+        doc["extensionsUsed"] = doc.get("extensionsUsed", []) + ["KHR_mesh_quantization"]
+        doc["extensionsRequired"] = ["KHR_mesh_quantization"]
     doc["accessors"], doc["bufferViews"] = accessors, views
     bin_len = sum(len(b) for b in blobs)
     doc["buffers"] = [{"byteLength": bin_len}]
@@ -581,6 +614,38 @@ def write_glb(path: str, mesh: dict) -> None:
             f.write(b)
 
 
+_GLB_COMPONENT = {np.int8: 5120, np.uint8: 5121, np.int16: 5122, np.uint16: 5123, np.uint32: 5125, np.float32: 5126}
+
+
+def _quantise_attributes(attrs: dict):
+    """write_glb(compact=True)'s attributes: each quantised one padded to a 4-byte multiple per element, and the node's
+    translation and scale that map the uint16 positions back to world coordinates.  The scale is one number, the bounding
+    box's largest extent, on all three axes: viewers transform NORMAL by the inverse transpose of the node matrix and TANGENT
+    by the matrix itself, and only a uniform scale leaves the directions the file stores pointing where they did."""
+    out = dict(attrs)
+    p = attrs["POSITION"].astype(np.float64)
+    lo = p.min(0) if len(p) else np.zeros(3)
+    ext = float((p.max(0) - lo).max()) if len(p) else 0.0
+    ext = ext if ext > 0 else 1.0
+    q = np.zeros((p.shape[0], 4), np.uint16)
+    q[:, :3] = np.clip(np.rint((p - lo) / ext * 65535.0), 0, 65535)
+    out["POSITION"] = q
+
+    def snorm8(a):
+        return np.clip(np.rint(a.astype(np.float64) * 127.0), -127, 127).astype(np.int8)
+    if "NORMAL" in attrs:
+        out["NORMAL"] = np.concatenate([snorm8(attrs["NORMAL"]), np.zeros((p.shape[0], 1), np.int8)], 1)
+    if "TANGENT" in attrs:
+        out["TANGENT"] = snorm8(attrs["TANGENT"])
+    if "COLOR_0" in attrs:
+        c = np.zeros((p.shape[0], 4), np.uint16)
+        c[:, :3] = np.rint(attrs["COLOR_0"].astype(np.float64) * 65535.0)
+        out["COLOR_0"] = c
+    # (x, y, z) -> (x, z, -y) of the low corner: the translation applied after the rotation
+    node = {"translation": [float(lo[0]), float(lo[2]), float(-lo[1])], "scale": [ext, ext, ext]}
+    return out, node
+
+
 def _cuda_u8(a) -> torch.Tensor:
     t = a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
     return t.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.uint8).contiguous()
@@ -590,7 +655,9 @@ def read_glb(path: str) -> dict:
     """Reads what :func:`write_glb` writes (numpy arrays), with :func:`read_obj`'s keys: vertices, faces (``arange`` for the
     per-face atlas's non-indexed primitive), normals, colors (sRGB bytes again), uv [F,3,2] (v up again; with ``uv_vertices``
     / ``uv_faces`` for an indexed textured primitive, the chart atlas), texture and normal_texture (RGB), and ``tangents``
-    [V,4].  Also ``"gltf"``, the JSON document."""
+    [V,4].  Also ``"gltf"``, the JSON document.  A compact file's quantised attributes come back dequantised as fp32 (glTF's
+    normalised-integer rule; positions through the node's scale and translation, in world coordinates again) and its JPEG
+    textures decoded by OpenCV."""
     import json
     import struct
     import cv2
@@ -612,13 +679,24 @@ def read_glb(path: str) -> dict:
 
     def accessor(i):
         a = doc["accessors"][i]
-        dt = {5126: np.float32, 5125: np.uint32}[a["componentType"]]
+        dt = np.dtype({v: k for k, v in _GLB_COMPONENT.items()}[a["componentType"]])
         k = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4}[a["type"]]
-        return np.frombuffer(view(a["bufferView"]), dt, count=a["count"] * k).reshape(a["count"], k).copy()
+        stride = doc["bufferViews"][a["bufferView"]].get("byteStride", k * dt.itemsize)
+        raw = np.frombuffer(view(a["bufferView"]), np.uint8, count=a["count"] * stride).reshape(a["count"], stride)
+        v = np.ascontiguousarray(raw[:, :k * dt.itemsize]).view(dt).reshape(a["count"], k)
+        if not a.get("normalized", False):
+            return v.copy()
+        m = float(np.iinfo(dt).max)
+        return np.maximum(v.astype(np.float64) / m, -1.0).astype(np.float32)
 
     prim = doc["meshes"][0]["primitives"][0]
     at = prim["attributes"]
     verts = accessor(at["POSITION"])
+    node = doc["nodes"][0]
+    if "scale" in node:
+        t = np.asarray(node.get("translation", [0.0, 0.0, 0.0]), np.float64)
+        lo = np.asarray([t[0], -t[2], t[1]])                    # the rotation undone: (x, y, z) <- (x, z, -y)
+        verts = (verts.astype(np.float64) * np.asarray(node["scale"], np.float64) + lo).astype(np.float32)
     faces = (accessor(prim["indices"]).reshape(-1, 3).astype(np.int32) if "indices" in prim
              else np.arange(verts.shape[0], dtype=np.int32).reshape(-1, 3))
     out = {"vertices": verts, "faces": faces, "gltf": doc}

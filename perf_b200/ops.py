@@ -1524,6 +1524,35 @@ def png_encode(image: torch.Tensor) -> bytes:
         return out[:n].cpu().numpy().tobytes()
 
 
+JPEG_MAX_SIDE = 65535       # SOF0's 16-bit height and width
+
+
+def jpeg_encode(image: torch.Tensor, quality: int) -> bytes:
+    """A baseline JPEG (JFIF, 4:4:4, the Annex K Huffman tables, a restart interval of one MCU row) of ``image`` [H,W,3] uint8
+    RGB, row 0 at the top, 1 <= H, W <= 65535, at IJG ``quality`` 1-100, coded on the GPU (``perf_jpeg_compress`` /
+    ``perf_jpeg_write``; include/perfb200.h states every byte): libjpeg's integer colour conversion, ISLOW DCT and
+    quantisation, so the file equals OpenCV's ``imencode`` with those settings byte for byte.  The host reads the file size,
+    allocates an output buffer of exactly that size, and copies the file."""
+    image = _chk(image, torch.uint8, "image")
+    if image.dim() != 3 or image.shape[2] != 3 or not 1 <= image.shape[0] <= JPEG_MAX_SIDE or not 1 <= image.shape[1] <= JPEG_MAX_SIDE:
+        raise ValueError(f"jpeg_encode: image {tuple(image.shape)}: needs [H,W,3] with 1 <= H, W <= {JPEG_MAX_SIDE}")
+    if isinstance(quality, bool) or int(quality) != quality or not 1 <= quality <= 100:
+        raise ValueError(f"jpeg_encode: quality {quality!r}: needs an integer in [1, 100]")
+    H, W, dev = image.shape[0], image.shape[1], image.device
+    ws = torch.empty(int(_L().perf_jpeg_workspace_bytes(H, W)), dtype=torch.uint8, device=dev)
+    size = torch.empty(1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        _call(_L().perf_jpeg_compress, _p(image), H, W, int(quality), _p(ws), ws.numel(), _stream(), launches=5)
+        _call(_L().perf_jpeg_file_bytes, _p(ws), ws.numel(), H, W, _p(size), _stream(), launches=0)
+        n = int(size.item())
+        out = torch.empty(n, dtype=torch.uint8, device=dev)
+        _call(_L().perf_jpeg_write, _p(ws), ws.numel(), H, W, _p(out), n, _p(size), _stream())
+        data = out.cpu().numpy().tobytes()
+        if int(size.item()) != n:
+            raise RuntimeError(f"jpeg_encode: perf_jpeg_write wrote {int(size.item())} bytes, perf_jpeg_file_bytes said {n}")
+        return data
+
+
 def corner_tangents(vertices: torch.Tensor, faces: torch.Tensor, normals: Optional[torch.Tensor], uv: torch.Tensor) -> torch.Tensor:
     """[F,3,3] fp32: per face corner the unit tangent of the frame the normal texture is baked and shaded with
     (``perf_mesh_corner_tangents``: MikkTSpace's t_k for per-face charts; the vertex ``normals``, else the geometric normal,

@@ -223,7 +223,10 @@ class CoreRunner:
         ``_fill`` last (``<stem>[_charts][_views]_fill.obj``), so an unfilled export is never overwritten; the PLY and the
         report do not change.  With ``mesh_glb: true`` the mesh is also written as one binary glTF file (``mesh.write_glb``:
         textures PNG-encoded on the GPU, normal texture with tangents), ``<OBJ stem>.glb`` when it has a texture, else
-        ``<PLY stem>.glb``; the other files do not change.  With ``mesh_report: true`` the written mesh
+        ``<PLY stem>.glb``; the other files do not change.  With ``mesh_glb_compact: true`` (which does not need
+        ``mesh_glb``) it is also written as ``<the same stem>_compact.glb`` (``write_glb(..., compact=True)``: JPEG textures
+        at ``mesh.GLB_JPEG_QUALITY``, ``KHR_mesh_quantization`` attributes), so an exact GLB is never overwritten; the other
+        files do not change.  With ``mesh_report: true`` the written mesh
         is then compared with the field (:meth:`mesh_report`): ``<stem>_report.json`` and ``<stem>_report_<i>.png``.  Returns
         (path, mesh) on rank 0, else (None, None)."""
         from .mesh import write_glb, write_obj, write_ply
@@ -280,6 +283,8 @@ class CoreRunner:
             write_obj(stem + ".obj", mesh)
         if bool(self.conf.get("mesh_glb", False)):
             write_glb(stem + ".glb", mesh)
+        if bool(self.conf.get("mesh_glb_compact", False)):
+            write_glb(stem + "_compact.glb", mesh, compact=True)
         if bool(self.conf.get("mesh_report", False)):
             self.mesh_report(mesh, path[:-len(".ply")], views=self.sup_pool if views else None)
         return path, mesh
