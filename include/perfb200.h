@@ -703,6 +703,65 @@ int perf_jpeg_file_bytes(const void* d_workspace, uint64_t workspace_bytes, int 
 int perf_jpeg_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
                     uint64_t* d_file_bytes, void* stream);
 
+/* ---- intra-only H.264 encoder (ops.h264_encode and perf_b200/video.py drive it; csrc/h264.cu).  d_frames [N,H,W,3] uint8
+ * RGB, row 0 at the top; 1 <= N <= 65535, H and W even in [2, 16384], at most 139264 macroblocks a frame (MaxFS of level
+ * 6.2), 0 <= qp <= 51, else PERF_EINVAL.  Every byte:
+ *   Stream: H.264 Constrained Baseline (profile_idc 66, constraint_set0_flag and constraint_set1_flag set), 8-bit 4:2:0,
+ *   CAVLC, one slice per picture.  Every frame is an IDR picture (nal_ref_idc 3), idr_pic_id = frame index & 1, frame_num 0,
+ *   pic_order_cnt_type 2, max_num_ref_frames 0, so every frame is coded at once and every MP4 sample is a sync sample.
+ *   Level: the smallest of Table A-1 (1 to 6.2, 1b skipped) whose MaxFS, MaxMBPS and sqrt(8 MaxFS) side bound admit the
+ *   frame at the frame rate (perf_h264_level; 0, and PERF_EINVAL from perf_h264_parameter_sets, beyond 6.2).  The bit rate is
+ *   not bounded by the level's MaxBR: constant QP decides it.
+ *   Size: the picture is ceil(W / 16) x ceil(H / 16) macroblocks, padded by repeating the last RGB column and row, and cropped
+ *   back with frame_cropping (right and bottom) in the SPS.
+ *   Colour: BT.601 limited range, Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16, Cb = ((-38 R - 74 G + 112 B + 128) >> 8) + 128,
+ *   Cr = ((112 R - 94 G - 18 B + 128) >> 8) + 128 (arithmetic shifts), per pixel; each chroma sample is (s0 + s1 + s2 + s3 + 2)
+ *   >> 2 of its 2 x 2 block.  The VUI carries video_full_range_flag 0, colour_primaries / transfer_characteristics /
+ *   matrix_coefficients 6 / 6 / 6 and timing_info (num_units_in_tick fps_den, time_scale 2 fps_num, fixed_frame_rate_flag 1).
+ *   PPS: CAVLC, pic_init_qp 26, chroma_qp_index_offset 0, deblocking_filter_control_present_flag 1.  Slice header:
+ *   slice_type 7 (I), slice_qp_delta qp - 26, disable_deblocking_filter_idc 1, so the decoder's output is exactly the
+ *   encoder's reconstruction (perf_h264_reconstruction).
+ *   Macroblocks: Intra 16x16 or Intra 4x4.  Intra 16x16: the luma mode (vertical, horizontal, DC, plane; those whose
+ *   neighbours exist) of least SATD + lambda bits(mb_type), SATD the sum over the 16 4x4 blocks of |Hadamard(source -
+ *   prediction)| / 2, bits 3 for vertical / horizontal and 5 for DC / plane, lambda = round(0.85 2^((qp - 12) / 6)), at least
+ *   1.  Intra 4x4: the blocks in decoding order, each the mode of the 9 (8.3.1.2; those whose neighbours exist, the top-right
+ *   samples replaced by p[3, -1] where 6.4.11.4 makes them unavailable) of least SATD + lambda (1 when it is the most
+ *   probable mode of 8.3.1.1, else 4), predicted from the reconstruction of the blocks before it; the macroblock's cost is
+ *   their sum + lambda, and Intra 4x4 is chosen when that is below the Intra 16x16 cost.  Its 4x4 blocks are quantised
+ *   whole (DC included) with the rounding term 2^qbits / 3; coded_block_pattern has one luma bit per 8x8 block with a
+ *   nonzero level, coded by the Intra_4x4 column of Table 9-4; mb_qp_delta is present only when it is nonzero.  The
+ *   chroma mode (DC,
+ *   horizontal, vertical, plane) of least SATD(Cb) + SATD(Cr) + lambda bits(intra_chroma_pred_mode), bits 1, 3, 3, 5; ties
+ *   go to the lower mode number.  Forward 4x4 core transform, quantised as sign(v) ((|v| MF + 2^qbits / 3) >> qbits), qbits
+ *   15 + qp / 6, MF of qp % 6 and the position class {13107, 5243, 8066} ...; the luma DCs by the 4x4 Hadamard, halved
+ *   (arithmetic shift), and the chroma DCs by the 2x2 one, both with MF of position 0, twice the rounding term and qbits + 1;
+ *   chroma at QPc of Table 8-15.  coded_block_pattern: luma 15 when any AC level is nonzero, else 0; chroma 2 when any AC
+ *   level, 1 when only DC levels are nonzero, else 0 (luma as above for Intra 16x16: 15 when any AC level is nonzero).  A macroblock whose CAVLC bits exceed 5934 (A.3.1: 128 + 3072 189 / 100)
+ *   or one of whose levels would need level_prefix > 15 is coded I_PCM with the source samples.
+ *   Integer arithmetic only; the only atomics are integer ORs, so the bytes do not depend on execution order.
+ * Calls, in order: perf_h264_workspace_bytes(N, H, W) bytes of d_workspace (16-byte aligned; per frame 384 bytes of
+ * reconstruction, 796 bytes of mode and levels and about 1.9 KB of slice data and staging per macroblock: about 11 bytes per
+ * pixel); perf_h264_encode (one launch per wavefront t = x + 2 y that holds a macroblock, at most ceil(W / 16) + 2 ceil(H / 16)
+ * - 2, then scan, emit, nal, finish); then
+ * perf_h264_au_bytes (each frame's access-unit size into d_au_bytes[0..N-1], a device-to-device copy) and, once the caller
+ * has read them, an output buffer of their sum; then perf_h264_write (1 launch and a copy): when the access units fit the
+ * out_bytes of d_out, frame after frame into d_out, each as a 4-byte big-endian length and the IDR NAL unit (AVCC, emulation
+ * prevention applied), and their total into d_total_bytes[0]; when they do not, nothing is written and d_total_bytes[0] is
+ * the size they need.  perf_h264_reconstruction: the decoder's output, N frames of I420 (Y [H,W], Cb, Cr [H/2,W/2]), into
+ * d_yuv.  perf_h264_mb_modes: per macroblock of every frame, raster order, 20 bytes: mode (0-3 the Intra 16x16 mode,
+ * 4 I_PCM, 5 Intra 4x4), the chroma mode, the luma and chroma coded_block_pattern, and the 16 Intra4x4PredMode values in
+ * raster order of the 4x4 blocks (2 outside Intra 4x4 macroblocks).  perf_h264_parameter_sets (host memory, no GPU): the SPS and PPS NAL units (header byte, no start code or length)
+ * for the frame size and fps_num / fps_den frames a second, back to back into out, their sizes into sps_bytes, pps_bytes. */
+int perf_h264_level(int H, int W, int fps_num, int fps_den);                  /* level_idc (10 .. 62), 0 outside the limits */
+int perf_h264_parameter_sets(int H, int W, int fps_num, int fps_den, uint8_t* out, int out_bytes, int* sps_bytes, int* pps_bytes);
+uint64_t perf_h264_workspace_bytes(int N, int H, int W);                      /* 0 outside the limits */
+int perf_h264_encode(const uint8_t* d_frames, int N, int H, int W, int qp, void* d_workspace, uint64_t workspace_bytes, void* stream);
+int perf_h264_au_bytes(const void* d_workspace, uint64_t workspace_bytes, int N, int H, int W, uint64_t* d_au_bytes, void* stream);
+int perf_h264_write(const void* d_workspace, uint64_t workspace_bytes, int N, int H, int W, uint8_t* d_out, uint64_t out_bytes,
+                    uint64_t* d_total_bytes, void* stream);
+int perf_h264_reconstruction(const void* d_workspace, uint64_t workspace_bytes, int N, int H, int W, uint8_t* d_yuv, void* stream);
+int perf_h264_mb_modes(const void* d_workspace, uint64_t workspace_bytes, int N, int H, int W, uint8_t* d_modes, void* stream);
+
 /* ---- fused training step (fixed-S sampler): forward with saves, composite backward, grid scatter ----
  * All per-sample buffers are SAMPLE-MAJOR: row = k * R + ray (k = sample index along the ray), so
  * that a warp of neighbouring rays reads/writes contiguous rows.  Replaces, for one optimisation

@@ -134,6 +134,14 @@ SIGNATURES = {
     "perf_jpeg_compress": (i32, [vp, i32, i32, i32, vp, u64, vp]),
     "perf_jpeg_write": (i32, [vp, u64, i32, i32, vp, u64, vp, vp]),
     "perf_jpeg_file_bytes": (i32, [vp, u64, i32, i32, vp, vp]),
+    "perf_h264_level": (i32, [i32, i32, i32, i32]),
+    "perf_h264_parameter_sets": (i32, [i32, i32, i32, i32, vp, i32, P(i32), P(i32)]),
+    "perf_h264_workspace_bytes": (u64, [i32, i32, i32]),
+    "perf_h264_encode": (i32, [vp, i32, i32, i32, i32, vp, u64, vp]),
+    "perf_h264_au_bytes": (i32, [vp, u64, i32, i32, i32, vp, vp]),
+    "perf_h264_write": (i32, [vp, u64, i32, i32, i32, vp, u64, vp, vp]),
+    "perf_h264_reconstruction": (i32, [vp, u64, i32, i32, i32, vp, vp]),
+    "perf_h264_mb_modes": (i32, [vp, u64, i32, i32, i32, vp, vp]),
     "perf_mesh_corner_tangents": (i32, [vp, u64, vp, u64, vp, vp, vp, vp]),
     "perf_train_forward": (i32, [P(RenderArgs), vp, vp, u64, i32, P(TrainBuffers), vp]),
     "perf_train_backward_composite": (i32, [i32, u32, u32, f32, f32, u64, vp, vp, P(TrainBuffers), vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -1553,6 +1553,66 @@ def jpeg_encode(image: torch.Tensor, quality: int) -> bytes:
         return data
 
 
+H264_MAX_SIDE = 16384
+H264_MAX_MBS = 139264       # MaxFS of level 6.2
+
+
+def h264_parameter_sets(H: int, W: int, fps: int = 30):
+    """(SPS, PPS) NAL units (header byte, no start code or length) of ``h264_encode``'s stream for H x W frames at ``fps``
+    frames a second (``perf_h264_parameter_sets``, host only)."""
+    out = (C.c_uint8 * 256)()
+    ns, np_ = C.c_int(0), C.c_int(0)
+    _lib.check(_L().perf_h264_parameter_sets(int(H), int(W), int(fps), 1, C.cast(out, C.c_void_p), 256, C.byref(ns), C.byref(np_)))
+    b = bytes(out)
+    return b[:ns.value], b[ns.value:ns.value + np_.value]
+
+
+def h264_encode(frames: torch.Tensor, qp: int, fps: int = 30, reconstruction: bool = False):
+    """H.264 Constrained Baseline of ``frames`` [N,H,W,3] uint8 RGB (row 0 at the top, H and W even), every frame an IDR
+    picture of Intra 16x16 / I_PCM macroblocks at constant ``qp`` 0-51, coded on the GPU (``perf_h264_encode`` /
+    ``perf_h264_write``; include/perfb200.h states every byte).  Returns (sps, pps, [access unit per frame]), each access unit
+    a 4-byte big-endian length and the IDR NAL unit (the MP4 sample); with ``reconstruction`` also the decoder's output,
+    [N, H W 3/2] uint8 I420 on the GPU (deblocking is off, so a conforming decoder returns exactly these samples)."""
+    frames = _chk(frames, torch.uint8, "frames")
+    if frames.dim() == 3:
+        frames = frames[None]
+    if frames.dim() != 4 or frames.shape[3] != 3 or frames.shape[0] < 1:
+        raise ValueError(f"h264_encode: frames {tuple(frames.shape)}: needs [N,H,W,3]")
+    N, H, W, dev = frames.shape[0], frames.shape[1], frames.shape[2], frames.device
+    if H % 2 or W % 2 or not 2 <= H <= H264_MAX_SIDE or not 2 <= W <= H264_MAX_SIDE or ((H + 15) // 16) * ((W + 15) // 16) > H264_MAX_MBS:
+        raise ValueError(f"h264_encode: frame {H} x {W}: needs even H and W in [2, {H264_MAX_SIDE}] and at most {H264_MAX_MBS} macroblocks")
+    if N > 65535:
+        raise ValueError(f"h264_encode: {N} frames in one call, at most 65535")
+    if isinstance(qp, bool) or int(qp) != qp or not 0 <= qp <= 51:
+        raise ValueError(f"h264_encode: qp {qp!r}: needs an integer in [0, 51]")
+    if isinstance(fps, bool) or int(fps) != fps or int(_L().perf_h264_level(H, W, int(fps), 1)) == 0:
+        raise ValueError(f"h264_encode: {H} x {W} at fps {fps!r}: needs a positive integer rate within level 6.2")
+    sps, pps = h264_parameter_sets(H, W, int(fps))
+    ws = torch.empty(int(_L().perf_h264_workspace_bytes(N, H, W)), dtype=torch.uint8, device=dev)
+    sizes = torch.empty(N, dtype=torch.int64, device=dev)
+    total = torch.empty(1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        MX, MY = (W + 15) // 16, (H + 15) // 16
+        waves = sum(1 for t in range(MX + 2 * MY - 2) if min(t // 2, MY - 1) >= max(0, (t - MX + 2) // 2))
+        _call(_L().perf_h264_encode, _p(frames), N, H, W, int(qp), _p(ws), ws.numel(), _stream(), launches=waves + 4)
+        _call(_L().perf_h264_au_bytes, _p(ws), ws.numel(), N, H, W, _p(sizes), _stream(), launches=0)
+        au = sizes.cpu().tolist()
+        out = torch.empty(sum(au), dtype=torch.uint8, device=dev)
+        _call(_L().perf_h264_write, _p(ws), ws.numel(), N, H, W, _p(out), out.numel(), _p(total), _stream())
+        rec = None
+        if reconstruction:
+            rec = torch.empty((N, H * W * 3 // 2), dtype=torch.uint8, device=dev)
+            _call(_L().perf_h264_reconstruction, _p(ws), ws.numel(), N, H, W, _p(rec), _stream(), launches=0)
+        data = out.cpu().numpy().tobytes()
+        if int(total.item()) != len(data):
+            raise RuntimeError(f"h264_encode: perf_h264_write wrote {int(total.item())} bytes, perf_h264_au_bytes said {len(data)}")
+    aus, o = [], 0
+    for n in au:
+        aus.append(data[o:o + n])
+        o += n
+    return (sps, pps, aus, rec) if reconstruction else (sps, pps, aus)
+
+
 def corner_tangents(vertices: torch.Tensor, faces: torch.Tensor, normals: Optional[torch.Tensor], uv: torch.Tensor) -> torch.Tensor:
     """[F,3,3] fp32: per face corner the unit tangent of the frame the normal texture is baked and shaded with
     (``perf_mesh_corner_tangents``: MikkTSpace's t_k for per-face charts; the vertex ``normals``, else the geometric normal,

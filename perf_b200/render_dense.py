@@ -7,7 +7,8 @@ the reference's unchanged Hydra YAML, with the panorama row-tiled over the ranks
 
 ``--poses``: [n,4,4] camera-to-world matrices (the reference builds them with its
 DenseTravelPoseSampler from the dataset's distance map, which is outside the hot path); without it
-a small circle of 8 poses around the origin is rendered.  Frames are written as PNG by rank 0.
+a small circle of 8 poses around the origin is rendered.  Frames are written as PNG by rank 0; with ``--video PATH``
+also as an H.264 MP4 coded on the GPU (``perf_b200.video``, at ``--qp``, default ``video.H264_QP``).
 """
 from __future__ import annotations
 
@@ -54,6 +55,9 @@ def main(argv=None):
     ap.add_argument("--height", type=int, default=512)
     ap.add_argument("--width", type=int, default=1024)
     ap.add_argument("--n-samples", type=int, default=128)
+    ap.add_argument("--video", default=None, help="also write the frames as an H.264 MP4 at this path")
+    ap.add_argument("--qp", type=int, default=None, help="constant QP of --video (0-51)")
+    ap.add_argument("--fps", type=int, default=30, help="frame rate of --video")
     ap.add_argument("overrides", nargs="*")
     args = ap.parse_args(argv)
     rank, world, local = parallel.init()
@@ -67,12 +71,20 @@ def main(argv=None):
     if rank == 0:
         os.makedirs(args.out, exist_ok=True)
     import cv2
+    video = None
+    if rank == 0 and args.video:
+        from .video import H264_QP, Mp4Writer
+        video = Mp4Writer(args.video, fps=args.fps, qp=H264_QP if args.qp is None else args.qp)
     for i, (rgb, dist) in enumerate(render_frames(renderer, poses, args.height, args.width, args.n_samples)):
         img = (rgb.clamp(0, 1) * 255).byte().cpu().numpy()[..., ::-1]
         cv2.imwrite(os.path.join(args.out, f"image_{i}.png"), img)
+        if video is not None:
+            video.add((rgb.clamp(0, 1) * 255).byte())
         inv = 1.0 / dist.clamp(min=1e-6)
         inv = (inv / inv.max() * 255).byte().cpu().numpy()
         cv2.imwrite(os.path.join(args.out, f"distance_{i}.png"), inv)
+    if video is not None:
+        video.close()
     if world > 1:
         import torch.distributed as dist_
         dist_.barrier()

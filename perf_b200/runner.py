@@ -162,12 +162,18 @@ class CoreRunner:
         """`core_exp_runner.py:223-246`.  With several ranks (torchrun) every frame is row-tiled over them and
         gathered on rank 0.  Returns the uint8 colour frames on rank 0 (the reference's ``color_frames``).
         Config key ``render_normals`` (default false): also write ``normal_{i}.png``, the weighted surface normal as
-        ``(n / |n| * 0.5 + 0.5) * 255`` (the reference's normal visualisation, `core_exp_runner.py:213`)."""
+        ``(n / |n| * 0.5 + 0.5) * 255`` (the reference's normal visualisation, `core_exp_runner.py:213`).
+        Config key ``render_video_h264`` (default false): also write ``video_h264.mp4``, the same frames as H.264 coded on the
+        GPU by rank 0 as they arrive (``video.Mp4Writer``), at constant QP ``render_video_qp`` (default ``video.H264_QP``)."""
         normals = bool(self.conf.get("render_normals", False))
         sampler = DenseTravelPoseSampler(self.pose_sampler, n_dense_poses=n_poses)
         out_dir = pjoin(self.exp_dir, "dense_images_new_" + cam_type)
         if self.is_main and write:
             os.makedirs(out_dir, exist_ok=True)
+        h264 = None
+        if self.is_main and write and bool(self.conf.get("render_video_h264", False)):
+            from .video import H264_QP, Mp4Writer
+            h264 = Mp4Writer(pjoin(out_dir, "video_h264.mp4"), qp=int(self.conf.get("render_video_qp", H264_QP)))
         rank, world = parallel.rank(), parallel.world_size()
         frames = []
         for i in range(sampler.n_poses):
@@ -189,6 +195,8 @@ class CoreRunner:
                 continue
             colors, distances = tile[..., :3], tile[..., 3:4]
             frames.append((colors.clip(0., 1.) * 255.).cpu().numpy().astype(np.uint8))
+            if h264 is not None:
+                h264.add((colors.clip(0., 1.) * 255.).to(torch.uint8))
             if write:
                 write_image(pjoin(out_dir, "image_{}.png".format(i)), colors * 255.)
                 write_image(pjoin(out_dir, "distance_{}.png".format(i)), colorize_single_channel_image(1. / distances))
@@ -198,6 +206,8 @@ class CoreRunner:
                     write_image(pjoin(out_dir, "normal_{}.png".format(i)), ((n * .5 + .5).clip(0., 1.) * 255.).byte())
         if self.is_main and write and frames:
             self._write_video(pjoin(out_dir, "video.mp4"), frames)
+        if h264 is not None and frames:
+            h264.close()
         return frames
 
     def export_mesh(self, resolution=None, threshold=None):
