@@ -496,6 +496,112 @@ __device__ __forceinline__ void wgmma_n32_ra_tb(float (&d)[16], const uint32_t* 
                    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+
+// ---------------------------------------------------------------- byte streams (png.cu, jpeg.cu, h264.cu)
+// Device: an atomic OR; host (the encoders' test harness builds and host-side writers): a plain one.
+__host__ __device__ __forceinline__ void or_u32(uint32_t* p, uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+    atomicOr(p, v);
+#else
+    *p |= v;
+#endif
+}
+__host__ __device__ __forceinline__ uint32_t bswap_u32(uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+    return __byte_perm(v, 0, 0x0123);
+#else
+    return __builtin_bswap32(v);
+#endif
+}
+// The bits v takes, 0 for 0
+__host__ __device__ __forceinline__ int bit_width(uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+    return 32 - __clz((int)v);
+#else
+    return v ? 32 - __builtin_clz(v) : 0;
+#endif
+}
+
+// Bit sinks of the MSB-first codes (JPEG, H.264): BitCount adds up lengths; MsbBits ORs the bits into words that are zero
+// where it writes, through a word-aligned 64-bit accumulator, one OR per 32 bits.  The words are stored byte-swapped, so on
+// a little-endian machine the buffer reads as bytes in stream order.  (Deflate is LSB-first: png.cu has its own writer.)
+struct BitCount {
+    uint32_t n = 0;
+    __host__ __device__ __forceinline__ void put(uint32_t, int nb) { n += nb; }
+};
+struct MsbBits {
+    uint32_t* out; int64_t base; uint64_t acc; int fill;
+    __host__ __device__ __forceinline__ MsbBits(uint32_t* o, int64_t pos) : out(o), base(pos & ~(int64_t)31), acc(0), fill((int)(pos & 31)) {}
+    // the low nb bits of v, 0 <= nb <= 32: shifted to the top of a word (the bits above them drop out), then to bit `fill`
+    __host__ __device__ __forceinline__ void put(uint32_t v, int nb)
+    {
+        if (nb == 0) return;
+        acc |= (uint64_t)(v << (32 - nb)) << (32 - fill);
+        fill += nb;
+        if (fill >= 32) {
+            or_u32(out + (base >> 5), bswap_u32((uint32_t)(acc >> 32)));
+            acc <<= 32; fill -= 32; base += 32;
+        }
+    }
+    __host__ __device__ __forceinline__ void flush()
+    {
+        if (fill > 0) or_u32(out + (base >> 5), bswap_u32((uint32_t)(acc >> 32)));
+    }
+    __host__ __device__ __forceinline__ int64_t pos() const { return base + fill; }     // the next bit's position
+};
+
+// Thread t's share [lo, hi) of n items over NT threads: contiguous runs of ceil(n / NT), the last ones short or empty.
+template <class I> struct ItemRange { I lo, hi; };
+template <int NT, class I>
+__host__ __device__ __forceinline__ ItemRange<I> thread_range(I n, int t)
+{
+    const I q = (n + NT - 1) / NT;
+    return {q * t < n ? q * t : n, q * (t + 1) < n ? q * (t + 1) : n};
+}
+
+// A CTA of NT threads that runs phases 0 .. NP - 1 of PHASE(args, shared state, CTA index, phase, thread) with a barrier
+// after each.  The state is static shared memory when it fits the 48 KB static limit, dynamic shared memory otherwise.
+constexpr size_t CTA_STATIC_SMEM = 48 * 1024;
+
+template <class A, class S, int NT, int NP, void (*PHASE)(const A&, S&, int64_t, int, int)>
+__global__ void __launch_bounds__(NT) cta_phases(const A a)
+{
+    S* s;
+    if constexpr (sizeof(S) <= CTA_STATIC_SMEM) {
+        __shared__ S static_smem;
+        s = &static_smem;
+    } else {
+        extern __shared__ __align__(16) uint8_t dynamic_smem[];
+        s = reinterpret_cast<S*>(dynamic_smem);
+    }
+    for (int p = 0; p < NP; ++p) {
+        PHASE(a, *s, blockIdx.x, p, threadIdx.x);
+        __syncthreads();
+    }
+}
+
+// n_ctas CTAs of cta_phases on stream st; the host harness runs every thread of each phase of each CTA in a serial loop.
+template <class A, class S, int NT, int NP, void (*PHASE)(const A&, S&, int64_t, int, int)>
+int run_cta_phases(const A& a, int64_t n_ctas, cudaStream_t st)
+{
+#ifdef PERF_HOST_HARNESS
+    (void)st;
+    S* s = new S();
+    for (int64_t c = 0; c < n_ctas; ++c)
+        for (int p = 0; p < NP; ++p)
+            for (int t = 0; t < NT; ++t) PHASE(a, *s, c, p, t);
+    delete s;
+#else
+    constexpr size_t dyn = sizeof(S) <= CTA_STATIC_SMEM ? 0 : sizeof(S);
+    if (dyn) PERF_CUDA(cudaFuncSetAttribute(cta_phases<A, S, NT, NP, PHASE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+    cta_phases<A, S, NT, NP, PHASE><<<(unsigned)n_ctas, NT, dyn, st>>>(a);
+    PERF_LAUNCH_CHECK();
+#endif
+    return PERF_OK;
+}
 #endif  // __CUDACC__
 
 }  // namespace perf

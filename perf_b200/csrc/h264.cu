@@ -60,56 +60,10 @@ struct H264Args {
     H264Tables tab;
 };
 
-__host__ __device__ __forceinline__ void h264_or(uint32_t* p, uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    atomicOr(p, v);
-#else
-    *p |= v;
-#endif
-}
-__host__ __device__ __forceinline__ uint32_t h264_bswap(uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    return __byte_perm(v, 0, 0x0123);
-#else
-    return __builtin_bswap32(v);
-#endif
-}
-__host__ __device__ __forceinline__ int h264_nbits(uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    return 32 - __clz((int)v);
-#else
-    return v ? 32 - __builtin_clz(v) : 0;
-#endif
-}
 __host__ __device__ __forceinline__ int h264_clip(int v) { return v < 0 ? 0 : v > 255 ? 255 : v; }
 
-// Bit sinks: H264Count adds up lengths, H264Bits ORs the bits into a slot, MSB first, one OR per 32 bits (word-aligned).
-struct H264Count {
-    uint32_t n = 0;
-    __host__ __device__ __forceinline__ void put(uint32_t, int nb) { n += nb; }
-};
-struct H264Bits {
-    uint32_t* out; int64_t base; uint64_t acc; int fill;
-    __host__ __device__ __forceinline__ H264Bits(uint32_t* o, int64_t pos) : out(o), base(pos & ~(int64_t)31), acc(0), fill((int)(pos & 31)) {}
-    __host__ __device__ __forceinline__ void put(uint32_t v, int nb)
-    {
-        if (nb == 0) return;
-        acc |= (uint64_t)(nb == 32 ? v : v & ((1u << nb) - 1u)) << (64 - fill - nb);
-        fill += nb;
-        if (fill >= 32) {
-            h264_or(out + (base >> 5), h264_bswap((uint32_t)(acc >> 32)));
-            acc <<= 32; fill -= 32; base += 32;
-        }
-    }
-    __host__ __device__ __forceinline__ void flush()
-    {
-        if (fill > 0) h264_or(out + (base >> 5), h264_bswap((uint32_t)(acc >> 32)));
-    }
-};
-template <class S> __host__ __device__ __forceinline__ void h264_ue(S& s, uint32_t v) { s.put(v + 1, 2 * h264_nbits(v + 1) - 1); }
+// Exp-Golomb codes (9.1) into a bit sink (common.cuh: BitCount, MsbBits)
+template <class S> __host__ __device__ __forceinline__ void h264_ue(S& s, uint32_t v) { s.put(v + 1, 2 * bit_width(v + 1) - 1); }
 template <class S> __host__ __device__ __forceinline__ void h264_se(S& s, int v) { h264_ue(s, v > 0 ? 2 * v - 1 : -2 * v); }
 
 // Raster index (x + 4 y) of 4x4 zigzag position k, and of luma4x4BlkIdx b's block in the macroblock
@@ -612,7 +566,7 @@ __host__ __device__ __forceinline__ void h264_mb(const H264Args& a, const H264Ta
         }
     }
     // ---- the exact bits; over the A.3.1 limit (or an uncodable level): I_PCM, reconstructed as the source
-    H264Count cnt;
+    BitCount cnt;
     const bool ok = h264_mb_syntax(cnt, tb, m, ml, mt, lev);
     if (!ok || cnt.n > (uint32_t)(PERF_H264_PCM_ABOVE_BITS)) {
         m.mode = 4; m.cmode = 0; m.cbp_l = 0; m.cbp_c = 0;
@@ -665,8 +619,8 @@ __host__ __device__ __forceinline__ uint32_t h264_after(const H264Args& a, int64
 
 __host__ __device__ __forceinline__ void h264_scan_phase(const H264Args& a, H264ScanSmem& s, int64_t f, int p, int t)
 {
-    const int64_t q = (a.M + H264_FRAME_THREADS - 1) / H264_FRAME_THREADS;
-    const int64_t m0 = q * t < a.M ? q * t : a.M, m1 = q * (t + 1) < a.M ? q * (t + 1) : a.M, base = f * a.M;
+    const auto [m0, m1] = thread_range<H264_FRAME_THREADS>(a.M, t);
+    const int64_t base = f * a.M;
     if (p == 0) {
         for (uint32_t ph = 0; ph < 8; ++ph) {
             uint32_t pos = ph;
@@ -675,7 +629,7 @@ __host__ __device__ __forceinline__ void h264_scan_phase(const H264Args& a, H264
         }
     } else if (p == 1) {
         if (t == 0) {
-            H264Count hc;
+            BitCount hc;
             h264_slice_header(hc, (int)f, a.qp);
             uint32_t off = hc.n;
             for (int j = 0; j < H264_FRAME_THREADS; ++j) { s.pre[j] = off; off += s.len[j][off & 7]; }
@@ -699,13 +653,13 @@ __host__ __device__ __forceinline__ void h264_emit(const H264Args& a, const H264
     const int mx = (int)(k % a.MX), my = (int)(k / a.MX);
     uint32_t* slot = (uint32_t*)(a.slots + f * a.slot);
     if (k == 0) {
-        H264Bits h(slot, 0);
+        MsbBits h(slot, 0);
         h264_slice_header(h, (int)f, a.qp);
         h.flush();
     }
     const H264Mb& m = a.mb[g];
     const uint32_t pos = a.moff[g];
-    H264Bits w(slot, pos);
+    MsbBits w(slot, pos);
     if (m.mode == 4) {
         h264_ue(w, 25);
         w.put(0, (int)((8 - ((pos + 9) & 7)) & 7));
@@ -741,8 +695,8 @@ struct H264NalSmem { uint32_t ins[H264_FRAME_THREADS][3]; uint8_t st[H264_FRAME_
 __host__ __device__ __forceinline__ void h264_nal_phase(const H264Args& a, H264NalSmem& s, int64_t f, int p, int t)
 {
     const uint8_t* src = a.slots + f * a.slot;
-    const int64_t n = a.fr[f].bits / 8, q = (n + H264_FRAME_THREADS - 1) / H264_FRAME_THREADS;
-    const int64_t i0 = q * t < n ? q * t : n, i1 = q * (t + 1) < n ? q * (t + 1) : n;
+    const int64_t n = a.fr[f].bits / 8;
+    const auto [i0, i1] = thread_range<H264_FRAME_THREADS>(n, t);
     if (p == 0) {
         for (int z0 = 0; z0 < 3; ++z0) {
             int z = z0;
@@ -810,30 +764,12 @@ __global__ void __launch_bounds__(H264_MB_THREADS) h264_mb_kernel(const H264Args
     if (g < n) h264_diag_mb(a, tb, g);
 }
 
-__global__ void __launch_bounds__(H264_FRAME_THREADS) h264_scan_kernel(const H264Args a)
-{
-    __shared__ H264ScanSmem s;
-    for (int p = 0; p < H264_SCAN_PHASES; ++p) {
-        h264_scan_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
 __global__ void __launch_bounds__(H264_MB_THREADS) h264_emit_kernel(const H264Args a)
 {
     __shared__ H264Tables tb;
     h264_load_tables(tb, a, H264_MB_THREADS);
     const int64_t g = (int64_t)blockIdx.x * H264_MB_THREADS + threadIdx.x;
     if (g < a.N * a.M) h264_emit(a, tb, g);
-}
-
-__global__ void __launch_bounds__(H264_FRAME_THREADS) h264_nal_kernel(const H264Args a)
-{
-    __shared__ H264NalSmem s;
-    for (int p = 0; p < H264_NAL_PHASES; ++p) {
-        h264_nal_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
 }
 
 __global__ void h264_finish_kernel(const H264Args a) { h264_finish(a); }
@@ -968,20 +904,18 @@ static int h264_args(H264Args& a, int N, int H, int W, void* ws, uint64_t ws_byt
     return PERF_OK;
 }
 
-// Host bit writer of the parameter sets, and the NAL unit around an RBSP (emulation prevention included)
-struct H264HostBits {
-    uint8_t b[64]; int n = 0;
-    H264HostBits() { memset(b, 0, sizeof(b)); }
-    __host__ __device__ void put(uint32_t v, int nb) { for (int i = nb - 1; i >= 0; --i, ++n) if ((v >> i) & 1) b[n >> 3] |= (uint8_t)(0x80 >> (n & 7)); }
-    void trailing() { put(1, 1); n = (n + 7) & ~7; }
-};
-static int h264_nal(uint8_t* out, int cap, uint8_t header, const H264HostBits& r)
+// The NAL unit around the RBSP that r wrote from bit 0 (rbsp_trailing_bits added here, emulation prevention included)
+static int h264_nal(uint8_t* out, int cap, uint8_t header, MsbBits& r)
 {
+    r.put(1, 1);
+    r.put(0, (int)((8 - (r.pos() & 7)) & 7));
+    r.flush();
+    const uint8_t* b = (const uint8_t*)r.out;
     int k = 0, z = 0;
     if (k < cap) out[k] = header;
     ++k;
-    for (int i = 0; i < r.n / 8; ++i) {
-        const uint8_t v = r.b[i];
+    for (int i = 0; i < r.pos() / 8; ++i) {
+        const uint8_t v = b[i];
         if (z == 2 && v <= 3) { if (k < cap) out[k] = 3; ++k; z = 0; }
         if (k < cap) out[k] = v;
         ++k;
@@ -1008,7 +942,8 @@ int perf_h264_parameter_sets(int H, int W, int fps_num, int fps_den, uint8_t* ou
     const int level = h264_level(H, W, fps_num, fps_den);
     PERF_CHECK_ARG(level > 0, "h264 %d x %d at %d / %d fps: beyond level 6.2 (Table A-1)", H, W, fps_num, fps_den);
     const int MX = (W + 15) / 16, MY = (H + 15) / 16;
-    H264HostBits s;
+    uint32_t sps[16] = {};                                            // 64 bytes: an SPS takes at most 26
+    MsbBits s(sps, 0);
     s.put(66, 8); s.put(0xC0, 8); s.put((uint32_t)level, 8);          // Constrained Baseline: constraint_set0 and 1
     h264_ue(s, 0);                                                    // seq_parameter_set_id
     h264_ue(s, 0);                                                    // log2_max_frame_num_minus4
@@ -1027,15 +962,14 @@ int perf_h264_parameter_sets(int H, int W, int fps_num, int fps_den, uint8_t* ou
     s.put(0, 1);                                                      // chroma_loc_info_present_flag
     s.put(1, 1); s.put((uint32_t)fps_den, 32); s.put(2u * (uint32_t)fps_num, 32); s.put(1, 1);   // timing_info, fixed frame rate
     s.put(0, 1); s.put(0, 1); s.put(0, 1); s.put(0, 1);               // nal_hrd, vcl_hrd, pic_struct, bitstream_restriction
-    s.trailing();
-    H264HostBits p;
+    uint32_t pps[16] = {};
+    MsbBits p(pps, 0);
     h264_ue(p, 0); h264_ue(p, 0);                                     // pic_parameter_set_id, seq_parameter_set_id
     p.put(0, 1); p.put(0, 1);                                         // CAVLC, bottom_field_pic_order_in_frame_present_flag
     h264_ue(p, 0); h264_ue(p, 0); h264_ue(p, 0);                      // num_slice_groups_minus1, num_ref_idx_l0 / l1 minus1
     p.put(0, 1); p.put(0, 2);                                         // weighted_pred_flag, weighted_bipred_idc
     h264_se(p, 0); h264_se(p, 0); h264_se(p, 0);                      // pic_init_qp_minus26, pic_init_qs_minus26, chroma_qp_index_offset
     p.put(1, 1); p.put(0, 1); p.put(0, 1);                            // deblocking_filter_control_present, constrained_intra_pred, redundant_pic_cnt
-    p.trailing();
     const int ns = h264_nal(out, out_bytes, 0x67, s);
     const int np = h264_nal(out + (ns < out_bytes ? ns : out_bytes), out_bytes - (ns < out_bytes ? ns : out_bytes), 0x68, p);
     *sps_bytes = ns; *pps_bytes = np;
@@ -1057,36 +991,28 @@ int perf_h264_encode(const uint8_t* d_frames, int N, int H, int W, int qp, void*
     a.rgb = d_frames; a.qp = qp;
     h264_tables(a.tab);
     const int T = a.MX + 2 * a.MY - 2;
+    const cudaStream_t st = (cudaStream_t)stream;
+    for (a.t = 0; a.t < T; ++a.t) {
+        const int64_t n = (int64_t)N * h264_diag_len(a);
 #ifdef PERF_HOST_HARNESS
-    (void)stream;
-    for (a.t = 0; a.t < T; ++a.t) {
-        const int64_t n = (int64_t)N * h264_diag_len(a);
         for (int64_t g = 0; g < n; ++g) h264_diag_mb(a, a.tab, g);
-    }
-    static H264ScanSmem ss;
-    for (int64_t f = 0; f < N; ++f)
-        for (int p = 0; p < H264_SCAN_PHASES; ++p)
-            for (int t = 0; t < H264_FRAME_THREADS; ++t) h264_scan_phase(a, ss, f, p, t);
-    for (int64_t g = 0; g < (int64_t)N * a.M; ++g) h264_emit(a, a.tab, g);
-    static H264NalSmem ns;
-    for (int64_t f = 0; f < N; ++f)
-        for (int p = 0; p < H264_NAL_PHASES; ++p)
-            for (int t = 0; t < H264_FRAME_THREADS; ++t) h264_nal_phase(a, ns, f, p, t);
-    h264_finish(a);
 #else
-    cudaStream_t st = (cudaStream_t)stream;
-    for (a.t = 0; a.t < T; ++a.t) {
-        const int64_t n = (int64_t)N * h264_diag_len(a);
         if (n == 0) continue;
         h264_mb_kernel<<<(unsigned)((n + H264_MB_THREADS - 1) / H264_MB_THREADS), H264_MB_THREADS, 0, st>>>(a, n);
         PERF_LAUNCH_CHECK();
+#endif
     }
-    h264_scan_kernel<<<(unsigned)N, H264_FRAME_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
+    rc = run_cta_phases<H264Args, H264ScanSmem, H264_FRAME_THREADS, H264_SCAN_PHASES, h264_scan_phase>(a, N, st); if (rc) return rc;
+#ifdef PERF_HOST_HARNESS
+    for (int64_t g = 0; g < (int64_t)N * a.M; ++g) h264_emit(a, a.tab, g);
+#else
     h264_emit_kernel<<<(unsigned)(((int64_t)N * a.M + H264_MB_THREADS - 1) / H264_MB_THREADS), H264_MB_THREADS, 0, st>>>(a);
     PERF_LAUNCH_CHECK();
-    h264_nal_kernel<<<(unsigned)N, H264_FRAME_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
+#endif
+    rc = run_cta_phases<H264Args, H264NalSmem, H264_FRAME_THREADS, H264_NAL_PHASES, h264_nal_phase>(a, N, st); if (rc) return rc;
+#ifdef PERF_HOST_HARNESS
+    h264_finish(a);
+#else
     h264_finish_kernel<<<1, 1, 0, st>>>(a);
     PERF_LAUNCH_CHECK();
 #endif

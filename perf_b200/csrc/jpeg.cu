@@ -42,31 +42,6 @@ struct JpegArgs {
     uint8_t hdr[JPEG_HEAD_BYTES];
 };
 
-__host__ __device__ __forceinline__ void jpeg_or(uint32_t* p, uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    atomicOr(p, v);
-#else
-    *p |= v;
-#endif
-}
-__host__ __device__ __forceinline__ uint32_t jpeg_bswap(uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    return __byte_perm(v, 0, 0x0123);
-#else
-    return __builtin_bswap32(v);
-#endif
-}
-__host__ __device__ __forceinline__ int jpeg_nbits(uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    return 32 - __clz((int)v);
-#else
-    return v ? 32 - __builtin_clz(v) : 0;
-#endif
-}
-
 // Natural (row-major) index of zigzag position k
 __host__ __device__ __forceinline__ int jpeg_zz(int k)
 {
@@ -135,56 +110,29 @@ __host__ __device__ __forceinline__ void jpeg_block(const JpegArgs& a, const Jpe
     }
 }
 
-// A word-aligned 64-bit accumulator over a row's slot, MSB first: one OR per 32 bits.
-struct JpegBits {
-    uint32_t* out; int64_t base; uint64_t acc; int fill;
-    __host__ __device__ __forceinline__ JpegBits(uint32_t* o, int64_t pos) : out(o), base(pos & ~(int64_t)31), acc(0), fill((int)(pos & 31)) {}
-    __host__ __device__ __forceinline__ void put(uint32_t v, int nb)
-    {
-        if (nb == 0) return;
-        acc |= (uint64_t)(v & ((1u << nb) - 1u)) << (64 - fill - nb);
-        fill += nb;
-        if (fill >= 32) {
-            jpeg_or(out + (base >> 5), jpeg_bswap((uint32_t)(acc >> 32)));
-            acc <<= 32; fill -= 32; base += 32;
-        }
-    }
-    __host__ __device__ __forceinline__ void flush()
-    {
-        if (fill > 0) jpeg_or(out + (base >> 5), jpeg_bswap((uint32_t)(acc >> 32)));
-    }
-};
-
-// The AC codes of one block (zigzag coefficients q): EMIT false returns their bits, true writes them.  libjpeg's
-// encode_one_block: per nonzero coefficient, ZRL (0xF0) per 16 zeros before it, then (run, size) and the size low bits of
-// v (v - 1 when negative); EOB (0x00) when the block ends in zeros.
-template <bool EMIT>
-__host__ __device__ __forceinline__ int jpeg_ac(const JpegTables& tb, int t, const int32_t q[64], JpegBits* w)
+// The AC codes of one block (zigzag coefficients q) into the bit sink s.  libjpeg's encode_one_block: per nonzero
+// coefficient, ZRL (0xF0) per 16 zeros before it, then (run, size) and the size low bits of v (v - 1 when negative); EOB
+// (0x00) when the block ends in zeros.
+template <class S>
+__host__ __device__ __forceinline__ void jpeg_ac(const JpegTables& tb, int t, const int32_t q[64], S& s)
 {
-    int bits = 0, r = 0;
+    int r = 0;
 #pragma unroll
     for (int k = 1; k < 64; ++k) {
         const int32_t v = q[k];
         if (v == 0) { ++r; continue; }
-        for (; r > 15; r -= 16) {
-            if (EMIT) w->put(tb.ac_code[t][0xF0], tb.ac_len[t][0xF0]);
-            else bits += tb.ac_len[t][0xF0];
-        }
-        const int nb = jpeg_nbits((uint32_t)(v < 0 ? -v : v)), sym = (r << 4) + nb;
-        if (EMIT) { w->put(tb.ac_code[t][sym], tb.ac_len[t][sym]); w->put((uint32_t)(v < 0 ? v - 1 : v), nb); }
-        else bits += tb.ac_len[t][sym] + nb;
+        for (; r > 15; r -= 16) s.put(tb.ac_code[t][0xF0], tb.ac_len[t][0xF0]);
+        const int nb = bit_width((uint32_t)(v < 0 ? -v : v)), sym = (r << 4) + nb;
+        s.put(tb.ac_code[t][sym], tb.ac_len[t][sym]);
+        s.put((uint32_t)(v < 0 ? v - 1 : v), nb);
         r = 0;
     }
-    if (r > 0) {
-        if (EMIT) w->put(tb.ac_code[t][0], tb.ac_len[t][0]);
-        else bits += tb.ac_len[t][0];
-    }
-    return bits;
+    if (r > 0) s.put(tb.ac_code[t][0], tb.ac_len[t][0]);
 }
 
 __host__ __device__ __forceinline__ int jpeg_dc_bits(const JpegTables& tb, int t, int32_t diff)
 {
-    const int nb = jpeg_nbits((uint32_t)(diff < 0 ? -diff : diff));
+    const int nb = bit_width((uint32_t)(diff < 0 ? -diff : diff));
     return tb.dc_len[t][nb] + nb;
 }
 
@@ -192,28 +140,28 @@ __host__ __device__ __forceinline__ int jpeg_dc_bits(const JpegTables& tb, int t
 __host__ __device__ __forceinline__ void jpeg_mcu_bits(const JpegArgs& a, const JpegTables& tb, int64_t m)
 {
     int32_t q[64];
-    uint32_t bits = 0;
+    BitCount bits;
     for (int c = 0; c < 3; ++c) {
         jpeg_block(a, tb, m, c, q);
         a.mdc[4 * m + c] = (int16_t)q[0];
-        bits += jpeg_ac<false>(tb, c > 0, q, nullptr);
+        jpeg_ac(tb, c > 0, q, bits);
     }
     a.mdc[4 * m + 3] = 0;
-    a.mbits[m] = bits;
+    a.mbits[m] = bits.n;
 }
 
 __host__ __device__ __forceinline__ void jpeg_mcu_emit(const JpegArgs& a, const JpegTables& tb, int64_t m)
 {
     const int bx = (int)(m % a.MX), by = (int)(m / a.MX);
-    JpegBits w((uint32_t*)(a.slots + by * a.slot), a.moff[m]);
+    MsbBits w((uint32_t*)(a.slots + by * a.slot), a.moff[m]);
     int32_t q[64];
     for (int c = 0; c < 3; ++c) {
         jpeg_block(a, tb, m, c, q);
         const int32_t diff = q[0] - (bx > 0 ? a.mdc[4 * (m - 1) + c] : 0);
-        const int nb = jpeg_nbits((uint32_t)(diff < 0 ? -diff : diff));
+        const int nb = bit_width((uint32_t)(diff < 0 ? -diff : diff));
         w.put(tb.dc_code[c > 0][nb], tb.dc_len[c > 0][nb]);
         w.put((uint32_t)(diff < 0 ? diff - 1 : diff), nb);
-        jpeg_ac<true>(tb, c > 0, q, &w);
+        jpeg_ac(tb, c > 0, q, w);
     }
     if (bx == a.MX - 1) {                       // the row's last byte is padded with 1 bits
         const int pad = (int)((8 - (a.rows[by].bits & 7)) & 7);
@@ -227,8 +175,7 @@ struct JpegRowSmem { uint32_t part[JPEG_ROW_THREADS], pre[JPEG_ROW_THREADS]; uin
 
 __host__ __device__ __forceinline__ void jpeg_row_phase(const JpegArgs& a, JpegRowSmem& s, int64_t by, int p, int t)
 {
-    const int q = (a.MX + JPEG_ROW_THREADS - 1) / JPEG_ROW_THREADS;
-    const int x0 = q * t < a.MX ? q * t : a.MX, x1 = q * (t + 1) < a.MX ? q * (t + 1) : a.MX;
+    const auto [x0, x1] = thread_range<JPEG_ROW_THREADS>(a.MX, t);
     const int64_t m0 = by * a.MX;
     if (p == 0) {
         uint32_t sum = 0;
@@ -285,9 +232,9 @@ __host__ __device__ __forceinline__ uint64_t jpeg_row_bytes(const JpegArgs& a, i
     return (a.rows[i].bits + 7) / 8 + a.rows[i].nff + (i < a.MY - 1 ? 2 : 0);
 }
 
-__host__ __device__ __forceinline__ void jpeg_finish_phase(const JpegArgs& a, JpegFinishSmem& s, int p, int t)
+__host__ __device__ __forceinline__ void jpeg_finish_phase(const JpegArgs& a, JpegFinishSmem& s, int64_t, int p, int t)
 {
-    const int64_t q = (a.MY + JPEG_THREADS - 1) / JPEG_THREADS, j0 = q * t < a.MY ? q * t : a.MY, j1 = q * (t + 1) < a.MY ? q * (t + 1) : a.MY;
+    const auto [j0, j1] = thread_range<JPEG_THREADS>((int64_t)a.MY, t);
     const int g = t >> 5;
     if (p == 0) {
         uint64_t b = 0;
@@ -332,8 +279,8 @@ __host__ __device__ __forceinline__ void jpeg_write_phase(const JpegArgs& a, Jpe
         return;
     }
     const uint8_t* src = a.slots + by * a.slot;
-    const int64_t n = (a.rows[by].bits + 7) / 8, q = (n + JPEG_THREADS - 1) / JPEG_THREADS;
-    const int64_t i0 = q * t < n ? q * t : n, i1 = q * (t + 1) < n ? q * (t + 1) : n;
+    const int64_t n = (a.rows[by].bits + 7) / 8;
+    const auto [i0, i1] = thread_range<JPEG_THREADS>(n, t);
     const int g = t >> 5;
     if (p == 0) {
         uint32_t k = 0;
@@ -376,15 +323,6 @@ __global__ void __launch_bounds__(JPEG_MCU_THREADS) jpeg_bits_kernel(const JpegA
     if (m < a.M) jpeg_mcu_bits(a, tb, m);
 }
 
-__global__ void __launch_bounds__(JPEG_ROW_THREADS) jpeg_row_kernel(const JpegArgs a)
-{
-    __shared__ JpegRowSmem s;
-    for (int p = 0; p < JPEG_ROW_PHASES; ++p) {
-        jpeg_row_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
 __global__ void __launch_bounds__(JPEG_MCU_THREADS) jpeg_emit_kernel(const JpegArgs a)
 {
     __shared__ JpegTables tb;
@@ -392,33 +330,6 @@ __global__ void __launch_bounds__(JPEG_MCU_THREADS) jpeg_emit_kernel(const JpegA
     __syncthreads();
     const int64_t m = (int64_t)blockIdx.x * JPEG_MCU_THREADS + threadIdx.x;
     if (m < a.M) jpeg_mcu_emit(a, tb, m);
-}
-
-__global__ void __launch_bounds__(JPEG_ROW_THREADS) jpeg_count_kernel(const JpegArgs a)
-{
-    __shared__ JpegCountSmem s;
-    for (int p = 0; p < JPEG_COUNT_PHASES; ++p) {
-        jpeg_count_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(JPEG_THREADS) jpeg_finish_kernel(const JpegArgs a)
-{
-    __shared__ JpegFinishSmem s;
-    for (int p = 0; p < JPEG_FINISH_PHASES; ++p) {
-        jpeg_finish_phase(a, s, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(JPEG_THREADS) jpeg_write_kernel(const JpegArgs a)
-{
-    __shared__ JpegWriteSmem s;
-    for (int p = 0; p < JPEG_WRITE_PHASES; ++p) {
-        jpeg_write_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
 }
 
 }  // namespace perf
@@ -560,36 +471,23 @@ int perf_jpeg_compress(const uint8_t* d_image, int H, int W, int quality, void* 
     PERF_CHECK_ARG(d_image, "NULL image");
     PERF_CHECK_ARG(quality >= 1 && quality <= 100, "jpeg quality %d: needs 1 <= quality <= 100", quality);
     jpeg_tables(a, quality);
+    const cudaStream_t st = (cudaStream_t)stream;
 #ifdef PERF_HOST_HARNESS
-    (void)stream;
     for (int64_t m = 0; m < a.M; ++m) jpeg_mcu_bits(a, a.tab, m);
-    static JpegRowSmem rs;
-    for (int64_t y = 0; y < a.MY; ++y)
-        for (int p = 0; p < JPEG_ROW_PHASES; ++p)
-            for (int t = 0; t < JPEG_ROW_THREADS; ++t) jpeg_row_phase(a, rs, y, p, t);
-    for (int64_t m = 0; m < a.M; ++m) jpeg_mcu_emit(a, a.tab, m);
-    static JpegCountSmem cs;
-    for (int64_t y = 0; y < a.MY; ++y)
-        for (int p = 0; p < JPEG_COUNT_PHASES; ++p)
-            for (int t = 0; t < JPEG_ROW_THREADS; ++t) jpeg_count_phase(a, cs, y, p, t);
-    static JpegFinishSmem fs;
-    for (int p = 0; p < JPEG_FINISH_PHASES; ++p)
-        for (int t = 0; t < JPEG_THREADS; ++t) jpeg_finish_phase(a, fs, p, t);
 #else
-    cudaStream_t st = (cudaStream_t)stream;
     const unsigned mcu_blocks = (unsigned)((a.M + JPEG_MCU_THREADS - 1) / JPEG_MCU_THREADS);
     jpeg_bits_kernel<<<mcu_blocks, JPEG_MCU_THREADS, 0, st>>>(a);
     PERF_LAUNCH_CHECK();
-    jpeg_row_kernel<<<(unsigned)a.MY, JPEG_ROW_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
+#endif
+    rc = run_cta_phases<JpegArgs, JpegRowSmem, JPEG_ROW_THREADS, JPEG_ROW_PHASES, jpeg_row_phase>(a, a.MY, st); if (rc) return rc;
+#ifdef PERF_HOST_HARNESS
+    for (int64_t m = 0; m < a.M; ++m) jpeg_mcu_emit(a, a.tab, m);
+#else
     jpeg_emit_kernel<<<mcu_blocks, JPEG_MCU_THREADS, 0, st>>>(a);
     PERF_LAUNCH_CHECK();
-    jpeg_count_kernel<<<(unsigned)a.MY, JPEG_ROW_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
-    jpeg_finish_kernel<<<1, JPEG_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
 #endif
-    return PERF_OK;
+    rc = run_cta_phases<JpegArgs, JpegCountSmem, JPEG_ROW_THREADS, JPEG_COUNT_PHASES, jpeg_count_phase>(a, a.MY, st); if (rc) return rc;
+    return run_cta_phases<JpegArgs, JpegFinishSmem, JPEG_THREADS, JPEG_FINISH_PHASES, jpeg_finish_phase>(a, 1, st);
 }
 
 int perf_jpeg_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
@@ -601,17 +499,8 @@ int perf_jpeg_write(const void* d_workspace, uint64_t workspace_bytes, int H, in
     PERF_CHECK_ARG(out_bytes >= (uint64_t)JPEG_HEAD_BYTES + 2, "output of %llu bytes, a JPEG takes more than %d",
                    (unsigned long long)out_bytes, JPEG_HEAD_BYTES + 2);
     a.out = d_out; a.out_bytes = out_bytes; a.size = d_file_bytes;
-#ifdef PERF_HOST_HARNESS
-    (void)stream;
-    static JpegWriteSmem ws;
-    for (int64_t y = 0; y <= a.MY; ++y)
-        for (int p = 0; p < JPEG_WRITE_PHASES; ++p)
-            for (int t = 0; t < JPEG_THREADS; ++t) jpeg_write_phase(a, ws, y, p, t);
-#else
-    jpeg_write_kernel<<<(unsigned)(a.MY + 1), JPEG_THREADS, 0, (cudaStream_t)stream>>>(a);
-    PERF_LAUNCH_CHECK();
-#endif
-    return PERF_OK;
+    return run_cta_phases<JpegArgs, JpegWriteSmem, JPEG_THREADS, JPEG_WRITE_PHASES, jpeg_write_phase>(a, a.MY + 1,
+                                                                                                    (cudaStream_t)stream);
 }
 
 int perf_jpeg_file_bytes(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint64_t* d_file_bytes, void* stream)

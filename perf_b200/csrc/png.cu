@@ -41,14 +41,6 @@ struct PngArgs {
     int64_t S;                                  // segments
 };
 
-__host__ __device__ __forceinline__ void png_or(uint32_t* p, uint32_t v)
-{
-#ifdef __CUDA_ARCH__
-    atomicOr(p, v);
-#else
-    *p |= v;
-#endif
-}
 __host__ __device__ __forceinline__ void png_inc(uint32_t* p)
 {
 #ifdef __CUDA_ARCH__
@@ -205,13 +197,13 @@ struct PngBits {
         acc |= (uint64_t)v << fill;
         fill += nb;
         if (fill >= 32) {
-            png_or(out + (base >> 5), (uint32_t)acc);
+            or_u32(out + (base >> 5), (uint32_t)acc);
             acc >>= 32; fill -= 32; base += 32;
         }
     }
     __host__ __device__ __forceinline__ void flush()
     {
-        if (fill > 0) png_or(out + (base >> 5), (uint32_t)acc);
+        if (fill > 0) or_u32(out + (base >> 5), (uint32_t)acc);
     }
 };
 
@@ -495,15 +487,15 @@ __host__ __device__ __forceinline__ void png_seg_phase(const PngArgs& a, PngSmem
                 PngBits w(s.out, s.hdr_bits + s.tok_bits);
                 w.put(s.code[256], s.len[256]);
                 w.flush();
-                png_or(s.out + ((s.m - 2) >> 2), 0xFFu << (8 * ((s.m - 2) & 3)));
-                png_or(s.out + ((s.m - 1) >> 2), 0xFFu << (8 * ((s.m - 1) & 3)));
+                or_u32(s.out + ((s.m - 2) >> 2), 0xFFu << (8 * ((s.m - 2) & 3)));
+                or_u32(s.out + ((s.m - 1) >> 2), 0xFFu << (8 * ((s.m - 1) & 3)));
             }
         }
     } else if (p == PNG_P_STORE) {
         const int m = s.m, words = (m + 3) >> 2;
         uint32_t* dst = (uint32_t*)(a.slots + c * PNG_SLOT);
         for (int i = t; i < words; i += PNG_THREADS) dst[i] = s.out[i];
-        const int q = (m + PNG_THREADS - 1) / PNG_THREADS, b0 = q * t < m ? q * t : m, b1 = q * (t + 1) < m ? q * (t + 1) : m;
+        const auto [b0, b1] = thread_range<PNG_THREADS>(m, t);
         s.crc[t] = png_crc_bytes(0, (const uint8_t*)s.out + b0, b1 - b0);
     } else if (p < PNG_P_FINAL) {
         const int k = p - PNG_P_CRC0, m = s.m, q = (m + PNG_THREADS - 1) / PNG_THREADS;
@@ -542,9 +534,9 @@ __host__ __device__ __forceinline__ void png_adler_cat(uint64_t& n, uint32_t& s1
 
 constexpr int64_t PNG_HEAD_BYTES = 8 + 25;      // signature, IHDR chunk
 
-__host__ __device__ __forceinline__ void png_finish_phase(const PngArgs& a, PngFinishSmem& s, int p, int t)
+__host__ __device__ __forceinline__ void png_finish_phase(const PngArgs& a, PngFinishSmem& s, int64_t, int p, int t)
 {
-    const int64_t q = (a.S + PNG_THREADS - 1) / PNG_THREADS, j0 = q * t < a.S ? q * t : a.S, j1 = q * (t + 1) < a.S ? q * (t + 1) : a.S;
+    const auto [j0, j1] = thread_range<PNG_THREADS>(a.S, t);
     const int g = t >> 5;
     if (p == 0) {
         uint64_t b = 0, n = 0; uint32_t s1 = 0, s2 = 0;
@@ -619,34 +611,6 @@ __host__ __device__ __forceinline__ void png_write_block(const PngArgs& a, int64
 }
 
 // ---------------------------------------------------------------- kernels
-__global__ void __launch_bounds__(PNG_FILTER_THREADS) png_filter_kernel(const PngArgs a)
-{
-    __shared__ PngFilterSmem s;
-    for (int p = 0; p < PNG_FILTER_PHASES; ++p) {
-        png_filter_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(PNG_THREADS) png_segment_kernel(const PngArgs a)
-{
-    extern __shared__ __align__(16) uint8_t png_smem[];
-    PngSmem& s = *(PngSmem*)png_smem;
-    for (int p = 0; p < PNG_SEG_PHASES; ++p) {
-        png_seg_phase(a, s, blockIdx.x, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(PNG_THREADS) png_finish_kernel(const PngArgs a)
-{
-    __shared__ PngFinishSmem s;
-    for (int p = 0; p < PNG_FINISH_PHASES; ++p) {
-        png_finish_phase(a, s, p, threadIdx.x);
-        __syncthreads();
-    }
-}
-
 __global__ void __launch_bounds__(PNG_THREADS) png_write_kernel(const PngArgs a)
 {
     png_write_block(a, blockIdx.x, threadIdx.x);
@@ -709,30 +673,10 @@ int perf_png_compress(const uint8_t* d_image, int H, int W, void* d_workspace, u
     PngArgs a;
     int rc = png_args(a, d_image, H, W, d_workspace, workspace_bytes); if (rc) return rc;
     PERF_CHECK_ARG(d_image, "NULL image");
-#ifdef PERF_HOST_HARNESS
-    (void)stream;
-    static PngFilterSmem fs;
-    for (int64_t y = 0; y < H; ++y)
-        for (int p = 0; p < PNG_FILTER_PHASES; ++p)
-            for (int t = 0; t < PNG_FILTER_THREADS; ++t) png_filter_phase(a, fs, y, p, t);
-    static PngSmem* ss = new PngSmem;
-    for (int64_t c = 0; c < a.S; ++c)
-        for (int p = 0; p < PNG_SEG_PHASES; ++p)
-            for (int t = 0; t < PNG_THREADS; ++t) png_seg_phase(a, *ss, c, p, t);
-    static PngFinishSmem gs;
-    for (int p = 0; p < PNG_FINISH_PHASES; ++p)
-        for (int t = 0; t < PNG_THREADS; ++t) png_finish_phase(a, gs, p, t);
-#else
-    cudaStream_t st = (cudaStream_t)stream;
-    png_filter_kernel<<<(unsigned)H, PNG_FILTER_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
-    PERF_CUDA(cudaFuncSetAttribute(png_segment_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PngSmem)));
-    png_segment_kernel<<<(unsigned)a.S, PNG_THREADS, sizeof(PngSmem), st>>>(a);
-    PERF_LAUNCH_CHECK();
-    png_finish_kernel<<<1, PNG_THREADS, 0, st>>>(a);
-    PERF_LAUNCH_CHECK();
-#endif
-    return PERF_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    rc = run_cta_phases<PngArgs, PngFilterSmem, PNG_FILTER_THREADS, PNG_FILTER_PHASES, png_filter_phase>(a, H, st); if (rc) return rc;
+    rc = run_cta_phases<PngArgs, PngSmem, PNG_THREADS, PNG_SEG_PHASES, png_seg_phase>(a, a.S, st); if (rc) return rc;
+    return run_cta_phases<PngArgs, PngFinishSmem, PNG_THREADS, PNG_FINISH_PHASES, png_finish_phase>(a, 1, st);
 }
 
 int perf_png_write(const void* d_workspace, uint64_t workspace_bytes, int H, int W, uint8_t* d_out, uint64_t out_bytes,
