@@ -1531,7 +1531,8 @@ def jpeg_encode(image: torch.Tensor, quality: int) -> bytes:
     """A baseline JPEG (JFIF, 4:4:4, the Annex K Huffman tables, a restart interval of one MCU row) of ``image`` [H,W,3] uint8
     RGB, row 0 at the top, 1 <= H, W <= 65535, at IJG ``quality`` 1-100, coded on the GPU (``perf_jpeg_compress`` /
     ``perf_jpeg_write``; include/perfb200.h states every byte): libjpeg's integer colour conversion, ISLOW DCT and
-    quantisation, so the file equals OpenCV's ``imencode`` with those settings byte for byte.  The host reads the file size,
+    quantisation, so the file equals OpenCV's ``imencode`` with those settings byte for byte.  A side above 65500 (libjpeg's
+    JPEG_MAX_DIMENSION) gives a valid baseline file that decoders built on libjpeg refuse to open.  The host reads the file size,
     allocates an output buffer of exactly that size, and copies the file."""
     image = _chk(image, torch.uint8, "image")
     if image.dim() != 3 or image.shape[2] != 3 or not 1 <= image.shape[0] <= JPEG_MAX_SIDE or not 1 <= image.shape[1] <= JPEG_MAX_SIDE:
